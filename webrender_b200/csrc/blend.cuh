@@ -336,3 +336,29 @@ WRD uint32_t wr_premult_over_pair(uint32_t dst_pair, uint32_t src_pair,
   uint32_t s = m + src_pair;                   // lanes <= 510
   return __vminu2(s, 0x00FF00FFu);             // saturating pack
 }
+
+// Premultiplied over with `+ src` folded into the addend k = 255 + 256*src: exact when every source lane
+// is <= src.a (the sum then cannot exceed 255).  See wr_fast_blend8.
+WRD uint32_t wr_over_folded(uint32_t dst_pair, uint32_t c, uint32_t k) {
+  return __byte_perm(dst_pair * c + k, 0, 0x4341);  // (t >> 8) & 0x00FF00FF
+}
+
+// One solid premultiplied-over layer on 8 pixels held as (B,R) / (G,A) pairs, with the layer's constants
+// from wr_solid_consts.  VALID: every source lane <= src.a (BatchInfo::premul_valid), no saturation needed.
+template <bool VALID>
+WRD void wr_fast_blend8(uint32_t* rb, uint32_t* ga, uint32_t c, uint32_t krb, uint32_t kga) {
+  if (VALID) {
+#pragma unroll
+    for (int p = 0; p < 8; p++) {
+      rb[p] = wr_over_folded(rb[p], c, krb);
+      ga[p] = wr_over_folded(ga[p], c, kga);
+    }
+  } else {
+    const uint32_t srb = (krb - 0x00FF00FFu) >> 8, sga = (kga - 0x00FF00FFu) >> 8;
+#pragma unroll
+    for (int p = 0; p < 8; p++) {
+      rb[p] = wr_premult_over_pair(rb[p], srb, c);
+      ga[p] = wr_premult_over_pair(ga[p], sga, c);
+    }
+  }
+}

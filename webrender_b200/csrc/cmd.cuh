@@ -123,5 +123,8 @@ struct BatchInfo {
   int all_copy;            // composite: 1 while no two commands of the batch overlap: CMD_COPY commands go to wr_composite_copy
   int glyph_ticket;        // text: next glyph wr_raster_glyphs hands to a warp
   int n_noncopy;           // composite: drawn commands that are not CMD_COPY (0: the tile kernel has nothing to do)
+  int cx0, cy0, cx1, cy1;  // common cover: the rect every drawn command contains (max of x0/y0, min of x1/y1);
+                           // reduced over the commands of simple batches only (see fold.cuh)
+  int fold_ticket;         // wr_fold_solid: CTAs that have written their partial tables (the last one composes them)
 };
 #define WR_ROW_TAB_MIN 4   // glyph rows (~12) too: the per-(command,row,tile) walk was a third of the text kernel

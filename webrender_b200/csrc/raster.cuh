@@ -21,6 +21,7 @@
 #include "texspan.cuh"
 #include "wrcu_internal.h"
 #include "repeat_add.cuh"
+#include "fold.cuh"
 
 struct RasterArgs {
   TargetDev tgt;
@@ -63,6 +64,8 @@ struct RasterArgs {
   int tmap_acquire;      // tensor-map table slots have been reused: acquire each map before use (tma.cuh)
   int pdl_early;         // programmatic dependent launch: this kernel may read its commands (written by the set-up
                          // launch, which finished earlier) before the kernel ahead of it in the stream has completed
+  uint8_t* fold;         // solid batches: the batch's 4 x 256 lookup tables (fold.cuh), written by wr_fold_solid
+                         // ahead of wr_raster_solid_premult; nullptr when no fold was launched
 };
 
 #define CHUNK_CMDS 256
@@ -793,9 +796,27 @@ static void wr_raster(const RasterArgs& a) {
     }
   }
 }
+static void wr_fold_solid(const RasterArgs& a) {
+  const BatchInfo bi = *a.info;
+  const int4 cov = wr_cover_tiles(bi, a.tgt);
+  if (!bi.simple || cov.z <= cov.x || cov.w <= cov.y) return;
+  wr_fold_host(a.hot, a.n, bi.premul_valid != 0, a.fold);
+}
+// Pixels of tiles inside the common cover go through the fold's tables (when one was launched), every
+// other pixel through the commands in batch order: disjoint pixel sets, so the order between them is free.
 static void wr_raster_solid_premult(const RasterArgs& a) {
   const BatchInfo bi = *a.info;
   if (!bi.simple) return;
+  int4 cov = make_int4(0, 0, 0, 0);
+  if (a.fold) {
+    cov = wr_cover_tiles(bi, a.tgt);
+    cov = make_int4(cov.x * WRCU_TILE_W, cov.y * WRCU_TILE_H, cov.z * WRCU_TILE_W, cov.w * WRCU_TILE_H);
+    if (cov.z <= cov.x || cov.w <= cov.y) cov = make_int4(0, 0, 0, 0);
+  }
+  for (int y = cov.y; y < cov.w; y++) {
+    uint32_t* rowp = (uint32_t*)(a.tgt.color + (size_t)y * a.tgt.color_pitch);
+    for (int x = cov.x; x < cov.z; x++) rowp[x] = wr_fold_px(a.fold, rowp[x]);
+  }
   for (int i = 0; i < a.n; i++) {
     const CmdHot c = a.hot[i];
     uint32_t srb = (uint32_t)c.col[0] | ((uint32_t)c.col[2] << 16), sga = (uint32_t)c.col[1] | ((uint32_t)c.col[3] << 16);
@@ -803,6 +824,7 @@ static void wr_raster_solid_premult(const RasterArgs& a) {
     for (int y = c.y0; y < c.y1; y++) {
       uint32_t* rowp = (uint32_t*)(a.tgt.color + (size_t)y * a.tgt.color_pitch);
       for (int x = c.x0; x < c.x1; x++) {
+        if (y >= cov.y && y < cov.w && x >= cov.x && x < cov.z) continue;
         uint32_t p = rowp[x];
         uint32_t rb = wr_premult_over_pair(p & 0x00FF00FFu, srb, cc);
         uint32_t ga = wr_premult_over_pair((p >> 8) & 0x00FF00FFu, sga, cc);
@@ -1332,28 +1354,6 @@ __global__ void __launch_bounds__(256) wr_depth_fail_rows(RasterArgs a, uint32_t
 #define FAST_THREADS 128
 #define FAST_CHUNK 128
 
-WRD uint32_t wr_over_folded(uint32_t dst_pair, uint32_t c, uint32_t k) {
-  return __byte_perm(dst_pair * c + k, 0, 0x4341);  // (t >> 8) & 0x00FF00FF
-}
-
-template <bool VALID>
-WRD void wr_fast_blend8(uint32_t* rb, uint32_t* ga, uint32_t c, uint32_t krb, uint32_t kga) {
-  if (VALID) {
-#pragma unroll
-    for (int p = 0; p < 8; p++) {
-      rb[p] = wr_over_folded(rb[p], c, krb);
-      ga[p] = wr_over_folded(ga[p], c, kga);
-    }
-  } else {
-    const uint32_t srb = (krb - 0x00FF00FFu) >> 8, sga = (kga - 0x00FF00FFu) >> 8;
-#pragma unroll
-    for (int p = 0; p < 8; p++) {
-      rb[p] = wr_premult_over_pair(rb[p], srb, c);
-      ga[p] = wr_premult_over_pair(ga[p], sga, c);
-    }
-  }
-}
-
 // `v0`, `v1`: this thread's pixels of the tile, loaded by the caller one tile ahead (software prefetch: the
 // loads of tile t+1 are in flight while tile t is classified and blended — a shallow batch is a
 // read-modify-write of the target at HBM speed, and the tile-at-a-time dependency chain
@@ -1375,10 +1375,8 @@ WRD void wr_fast_tile(const RasterArgs& a, int tx0, int ty0, uint4* fa, int4* fb
     if (base + (int)threadIdx.x < a.n) {
       const CmdHot c = a.hot[base + threadIdx.x];
       keep = c.x1 > tx0 && c.x0 < tx0 + WRCU_TILE_W && c.y1 > ty0 && c.y0 < ty0 + WRCU_TILE_H && c.x1 > c.x0;
-      const uint32_t full = c.x0 <= tx0 && c.x1 >= tx0 + WRCU_TILE_W && c.y0 <= ty0 && c.y1 >= ty0 + WRCU_TILE_H;
-      const uint32_t srb = (uint32_t)c.col[0] | ((uint32_t)c.col[2] << 16);  // B | R<<16
-      const uint32_t sga = (uint32_t)c.col[1] | ((uint32_t)c.col[3] << 16);  // G | A<<16
-      A = make_uint4(255u - c.col[3], 0x00FF00FFu + (srb << 8), 0x00FF00FFu + (sga << 8), full);
+      A = wr_solid_consts(c);
+      A.w = c.x0 <= tx0 && c.x1 >= tx0 + WRCU_TILE_W && c.y0 <= ty0 && c.y1 >= ty0 + WRCU_TILE_H;  // full cover
       B = make_int4(c.x0, c.x1, c.y0, c.y1);
     }
     const unsigned bal = __ballot_sync(0xFFFFFFFFu, keep);
@@ -1511,11 +1509,83 @@ __global__ void __launch_bounds__(FLAT_THREADS) wr_raster_solid_flat(RasterArgs 
   }
 }
 
+// ---- the lookup tables of a solid batch (fold.cuh) -----------------------------------------------------
+// WR_FOLD_CTAS CTAs; warp w of CTA b folds segment b * WR_FOLD_SEGS + w of the command list over the 256
+// inputs (lane l holds inputs 8l .. 8l+7 of all four channels as 16-bit lane pairs and applies the tile
+// kernel's blend to them).  Each CTA composes its segment tables into a partial table; the last CTA to
+// finish (a ticket in BatchInfo: no CTA ever waits for another) composes the partial tables in batch order.
+// The work is n x 512 lane-pair multiply-adds and as many byte permutes: on one SM's integer pipes
+// (64 per clock) 16 clocks per command: 8 us for config B's 1000 layers on one CTA; spread over 8 SMs, 1 us.
+// Returns at once unless the batch is simple and a whole tile lies inside the common cover, the only place
+// wr_raster_solid_premult reads the tables.
+#define FOLD_THREADS (WR_FOLD_SEGS * 32)
+static_assert(FOLD_THREADS == WR_FOLD_ENTRIES, "wr_fold_solid composes one table entry per thread");
+static_assert(FAST_THREADS * 8 == WR_FOLD_ENTRIES, "wr_raster_solid_premult loads the tables 8 bytes per thread");
+
+template <bool VALID>
+__device__ __forceinline__ void wr_fold_warp(const CmdHot* hot, int s0, int s1, uint32_t* rb, uint32_t* ga) {
+  const int lane = threadIdx.x & 31;
+  for (int base = s0; base < s1; base += 32) {
+    // 32 commands per round, loaded one per lane and handed to the whole warp by shuffles
+    uint4 k = make_uint4(0, 0, 0, 0);
+    bool keep = false;
+    if (base + lane < s1) {
+      const CmdHot c = hot[base + lane];
+      keep = c.x1 > c.x0;  // what the tile kernel keeps: commands that draw nothing stay identity
+      k = wr_solid_consts(c);
+    }
+    unsigned m = __ballot_sync(0xFFFFFFFFu, keep);
+    while (m) {
+      const int src = __ffs((int)m) - 1;
+      m &= m - 1;
+      wr_fast_blend8<VALID>(rb, ga, __shfl_sync(0xFFFFFFFFu, k.x, src), __shfl_sync(0xFFFFFFFFu, k.y, src),
+                            __shfl_sync(0xFFFFFFFFu, k.z, src));
+    }
+  }
+}
+
+static_assert(WR_FOLD_CTAS * WR_FOLD_ENTRIES == FOLD_THREADS * 8, "the last CTA loads the partial tables 8 bytes per thread");
+
+__global__ void __launch_bounds__(FOLD_THREADS) wr_fold_solid(RasterArgs a) {
+  __shared__ __align__(16) uint8_t segs[WR_FOLD_SEGS * WR_FOLD_ENTRIES];
+  __shared__ int s_last;
+  wr_pdl_launch_dependents();
+  wr_pdl_wait();
+  const BatchInfo bi = *a.info;
+  const int4 cov = wr_cover_tiles(bi, a.tgt);
+  if (!bi.simple || cov.z <= cov.x || cov.w <= cov.y) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nseg = wr_fold_nseg(a.n), seg0 = blockIdx.x * WR_FOLD_SEGS;
+  if (seg0 + warp < nseg) {
+    int s0, s1;
+    wr_fold_segment(a.n, nseg, seg0 + warp, &s0, &s1);
+    uint32_t rb[8], ga[8];
+    wr_fold_init(rb, ga, lane * 8);
+    if (bi.premul_valid) wr_fold_warp<true>(a.hot, s0, s1, rb, ga);
+    else wr_fold_warp<false>(a.hot, s0, s1, rb, ga);
+    wr_fold_store(rb, ga, lane * 8, segs + warp * WR_FOLD_ENTRIES);
+  }
+  __syncthreads();
+  uint8_t* part = a.fold + WR_FOLD_ENTRIES;  // the CTAs' partial tables, in CTA order
+  part[blockIdx.x * WR_FOLD_ENTRIES + threadIdx.x] =
+      wr_fold_compose(segs, min(max(nseg - seg0, 0), WR_FOLD_SEGS), threadIdx.x);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(const_cast<int*>(&a.info->fold_ticket), 1) == WR_FOLD_CTAS - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  ((uint2*)segs)[threadIdx.x] = __ldcg((const uint2*)part + threadIdx.x);  // written by other CTAs: from L2
+  __syncthreads();
+  a.fold[threadIdx.x] = wr_fold_compose(segs, WR_FOLD_CTAS, threadIdx.x);
+}
+
 __global__ void __launch_bounds__(FAST_THREADS)
 wr_raster_solid_premult(RasterArgs a) {
   __shared__ uint4 fa[FAST_CHUNK];
   __shared__ int4 fb[FAST_CHUNK];
   __shared__ int wsum[FAST_THREADS / 32];
+  __shared__ __align__(16) uint8_t lut[WR_FOLD_ENTRIES];
   wr_pdl_launch_dependents();
   wr_pdl_wait();
   const BatchInfo bi = *a.info;
@@ -1529,16 +1599,34 @@ wr_raster_solid_premult(RasterArgs a) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   auto tile_px = [&](int t, int row) {  // this thread's 16 bytes of row `row` (0 / 1 → tile rows warp, warp + 4)
     const int tx0 = (bx0 + t % nx) * WRCU_TILE_W, ty0 = (by0 + t / nx) * WRCU_TILE_H;
-    return (const uint4*)(a.tgt.color + (size_t)(ty0 + warp + 4 * row) * a.tgt.color_pitch + (size_t)(tx0 + lane * 4) * 4);
+    return (uint4*)(a.tgt.color + (size_t)(ty0 + warp + 4 * row) * a.tgt.color_pitch + (size_t)(tx0 + lane * 4) * 4);
   };
   int t = blockIdx.x;
   uint4 n0 = make_uint4(0, 0, 0, 0), n1 = n0;
   if (t < n_tiles) { n0 = *tile_px(t, 0); n1 = *tile_px(t, 1); }
+  // Tiles wholly inside the common cover take the fold's tables (when wr_fold_solid ran ahead of this kernel).
+  // Their tile range stays in shared memory and is re-read per tile: held in registers through the tile loop
+  // it takes the kernel from 72 to 80 registers, one resident CTA per SM fewer.
+  __shared__ int s_cov[4];
+  {
+    const int4 c = a.fold ? wr_cover_tiles(bi, a.tgt) : make_int4(0, 0, 0, 0);
+    if (threadIdx.x == 0) { s_cov[0] = c.x; s_cov[1] = c.y; s_cov[2] = c.z; s_cov[3] = c.w; }
+    if (c.z > c.x && c.w > c.y) ((uint2*)lut)[threadIdx.x] = ((const uint2*)a.fold)[threadIdx.x];
+  }
+  __syncthreads();
+  const volatile int* cov = s_cov;
   for (; t < n_tiles; t += gridDim.x) {
     const uint4 v0 = n0, v1 = n1;
     const int tn = t + gridDim.x;
     if (tn < n_tiles) { n0 = *tile_px(tn, 0); n1 = *tile_px(tn, 1); }  // next tile: issued now, used next iteration
-    const int tx0 = (bx0 + t % nx) * WRCU_TILE_W, ty0 = (by0 + t / nx) * WRCU_TILE_H;
+    const int tx = bx0 + t % nx, ty = by0 + t / nx;
+    if (tx >= cov[0] && tx < cov[2] && ty >= cov[1] && ty < cov[3]) {
+      // every command of the batch covers this tile: the layers are the tables (no chunk classification)
+      *tile_px(t, 0) = make_uint4(wr_fold_px(lut, v0.x), wr_fold_px(lut, v0.y), wr_fold_px(lut, v0.z), wr_fold_px(lut, v0.w));
+      *tile_px(t, 1) = make_uint4(wr_fold_px(lut, v1.x), wr_fold_px(lut, v1.y), wr_fold_px(lut, v1.z), wr_fold_px(lut, v1.w));
+      continue;
+    }
+    const int tx0 = tx * WRCU_TILE_W, ty0 = ty * WRCU_TILE_H;
     if (bi.premul_valid) wr_fast_tile<true>(a, tx0, ty0, fa, fb, wsum, v0, v1);
     else wr_fast_tile<false>(a, tx0, ty0, fa, fb, wsum, v0, v1);
   }

@@ -66,6 +66,9 @@ WRD void wr_reset_batch_info(BatchInfo* info) {
   info->all_copy = 1;
   info->glyph_ticket = 0;
   info->n_noncopy = 0;
+  info->cx0 = -0x7fffffff; info->cy0 = -0x7fffffff;
+  info->cx1 = 0x7fffffff; info->cy1 = 0x7fffffff;
+  info->fold_ticket = 0;
 }
 // Each setup kernel also re-arms the per-batch record the NEXT draw will use
 // (records rotate through a ring of 4; the one after the current was last read
@@ -738,6 +741,10 @@ WRD_SHARED bool wr_emit_quad(const SetupArgs& a, int idx, const QuadOut& q, int*
     if (!(h.col[0] <= h.col[3] && h.col[1] <= h.col[3] && h.col[2] <= h.col[3])) a.info->premul_valid = 0;
     atomicMin(&a.info->bx0, (int)h.x0); atomicMin(&a.info->by0, (int)h.y0);
     atomicMax(&a.info->bx1, (int)h.x1); atomicMax(&a.info->by1, (int)h.y1);
+    if (simple) {  // the common cover is read only while the whole batch is simple
+      atomicMax(&a.info->cx0, (int)h.x0); atomicMax(&a.info->cy0, (int)h.y0);
+      atomicMin(&a.info->cx1, (int)h.x1); atomicMin(&a.info->cy1, (int)h.y1);
+    }
     if (a.tile_mask) {
       const int tx_a = max((int)h.x0, 0) / WRCU_TILE_W, tx_b = (min((int)h.x1, a.tgt.w) + WRCU_TILE_W - 1) / WRCU_TILE_W;
       const int ty_a = max((int)h.y0, 0) / WRCU_TILE_H, ty_b = (min((int)h.y1, a.tgt.h) + WRCU_TILE_H - 1) / WRCU_TILE_H;

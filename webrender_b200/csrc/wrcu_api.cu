@@ -297,6 +297,13 @@ extern "C" int wrcu_ctx_create(int device_ordinal, wrcu_ctx** out) {
 #ifndef WRCU_HOSTEMU
     if (c->flat_max > FLAT_MAX) c->flat_max = FLAT_MAX;
 #endif
+    // deeper solid batches fold their layers into lookup tables first (wr_fold_solid, one extra launch), worth it
+    // once the tile kernel's per-layer work outweighs the fold's fixed cost.  bench.py's sweep on an H100 SXM
+    // (raster kernel time, the fold included): 4 layers 26.7-27.2 us tiled vs 28.3 folded, 8 layers 30.8-31.3
+    // tiled vs 29.5-30.0 folded.  WRCU_FOLD_MIN overrides it for that measurement.
+    e = getenv("WRCU_FOLD_MIN");
+    c->fold_min = e ? atoi(e) : 8;
+    if (c->fold_min < 1) c->fold_min = 1;
   }
   c->row_cap = 16 << 20;  // 64 MiB of row tables per batch; commands beyond it fall back to walking
   if (cudaMalloc((void**)&c->row_tab, (size_t)c->row_cap * sizeof(float)) != cudaSuccess) {
@@ -338,6 +345,7 @@ extern "C" void wrcu_ctx_destroy(wrcu_ctx* c) {
   if (c->cmd_hot) cudaFree(c->cmd_hot);
   if (c->cmd_cold) cudaFree(c->cmd_cold);
   if (c->batch_info) cudaFree(c->batch_info);
+  if (c->fold_lut) cudaFree(c->fold_lut);
   if (c->pool_ctr) cudaFree(c->pool_ctr);
   for (cudaStream_t st : c->side) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
   for (cudaEvent_t e : c->op_events) cudaEventDestroy(e);
@@ -1843,8 +1851,18 @@ static int launch_raster(wrcu_ctx* c, PendingOp& op) {
                  ra.depth_mode == WRCU_DEPTH_OFF &&
                  (kind == WRCU_KIND_QUAD_TEXTURED || kind == WRCU_KIND_BRUSH_SOLID);  // the only kinds that emit CMD_CONST_COLOR
   ra.fast_eligible = fast_ok ? 1 : 0;
+  ra.fold = nullptr;
   if (fast_ok) {
+    // this batch's tables sit in the slot of its BatchInfo record, so batches queued on side streams never share one
+    // (allocated with the first batch that folds)
+    if (n >= c->fold_min && !c->fold_lut)
+      WRCU_CUDA(c, cudaMalloc((void**)&c->fold_lut, 2 * (size_t)wrcu_ctx::QMAX * WR_FOLD_SLOT));
+    uint8_t* fold = c->fold_lut ? c->fold_lut + (size_t)(ra.info - (const BatchInfo*)c->batch_info) * WR_FOLD_SLOT : nullptr;
 #ifdef WRCU_HOSTEMU
+    if (n >= c->fold_min) {
+      ra.fold = fold;
+      wr_fold_solid(ra);
+    }
     wr_raster_solid_premult(ra);
 #else
     // persistent CTAs: size the grid so the tile count splits evenly over the
@@ -1875,6 +1893,11 @@ static int launch_raster(wrcu_ctx* c, PendingOp& op) {
         const double eff = (double)n_tiles / ((double)rounds * slots);
         if (eff > best_eff + 1e-9) { best_eff = eff; best_grid = slots; }
       }
+    }
+    if (n >= c->fold_min) {
+      ra.fold = fold;
+      wr_launch_chain(c, wr_fold_solid, (unsigned)WR_FOLD_CTAS, FOLD_THREADS, 0, ra);
+      c->stats.kernel_launches++;
     }
     wr_launch_chain(c, wr_raster_solid_premult, (unsigned)best_grid, FAST_THREADS, 0, ra);
     }

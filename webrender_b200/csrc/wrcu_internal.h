@@ -10,6 +10,7 @@
 //   raster.cuh       Tile-resident raster kernels: one CTA owns a 128x8-pixel
 //                    framebuffer tile, keeps it in registers, walks the batch's
 //                    commands IN ORDER, blends, and writes the tile once.
+//   fold.cuh         Solid batches as per-channel lookup tables (wr_fold_solid).
 //   setup_*.cuh      Vertex stages per BatchKind.
 #pragma once
 
@@ -146,6 +147,8 @@ struct wrcu_ctx {
   float* row_tab = nullptr;      // row-table pool of the current batch (CmdCold::row_off)
   int row_cap = 0;               // floats
   int flat_max = 2;          // solid batches of <= flat_max layers take the streaming kernel
+  int fold_min = 0;          // solid batches of >= fold_min layers get lookup tables (wr_fold_solid) for full-cover tiles
+  uint8_t* fold_lut = nullptr;  // those tables (WR_FOLD_SLOT bytes per BatchInfo record), indexed like batch_info
   int fast_ctas_per_sm = 0;  // resident CTAs/SM of the solid-premult kernel (occupancy API)
   // TMA: one 128-byte CUtensorMap per RGBA8 texture (box 256x16 px), built on the host at texture
   // creation (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint) and kept in a device table
