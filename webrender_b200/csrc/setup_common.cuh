@@ -123,7 +123,7 @@ WRD_SHARED void wr_fill_row_edge(const SetupArgs& a, int cidx, int e) {
 #define WR_ROW_TAB_TALL 512
 #ifdef WRCU_HOSTEMU
 #define WR_SETUP_KERNEL(name)                                     \
-  static void name(const SetupArgs& a) {                          \
+  static void name##_block(const SetupArgs& a, int) {             \
     if (a.info_next) wr_reset_batch_info(a.info_next);            \
     for (int i = 0; i < a.n; i++) {                               \
       name##_one(a, i);                                           \

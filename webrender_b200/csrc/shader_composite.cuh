@@ -11,6 +11,8 @@
 //          g[12..19] the instance's sColor0 view (tile lists carry one texture per instance)
 WRD const TexView& wr_composite_tex(const CmdCold& k) { return *(const TexView*)&k.g[12]; }
 static_assert(sizeof(TexView) <= 32, "TexView must fit CmdCold::g[12..19]");
+// The most commands the copy kernel (wr_composite_copy) stages; the host keeps longer tile lists on the tile kernel.
+#define WR_COPY_MAX_CMDS 128
 struct CompositeShader {
   struct Row {
     float o[2], step[2];
@@ -231,7 +233,6 @@ __device__ __noinline__ void wr_setup_composite_block(const SetupArgs& a, int id
 //     thread 0 bulk-stores the destination box and refills the slot that has just drained.
 // The batch's copy commands, staged once per CTA into shared memory (index-preserving, so every CTA deals
 // the boxes the same way): rect, source origin, the source's tensor map and plain view.
-#define WR_COPY_MAX_CMDS 128
 struct WrCopyCmd {
   short x0, y0;
   int w, h;        // 0 x 0: not a copy command

@@ -1449,6 +1449,110 @@ static int ensure_cmd_capacity(wrcu_ctx* c, size_t n) {
   return WRCU_OK;
 }
 
+#ifndef WRCU_HOSTEMU
+// A raster-class launch with programmatic stream serialization (see raster.cuh wr_pdl_wait); the ordinary
+// launch when the context has it switched off (WRCU_PDL=0).
+template <typename K>
+static void wr_launch_chain(wrcu_ctx* c, K kernel, unsigned grid, unsigned block, size_t smem, const RasterArgs& ra) {
+  // (a launch that directly follows an event wait in its stream is an ordinary one: the programmatic edge is
+  // between two kernels, and nothing is gained by leaving it to the driver what an event wait in between means)
+  if (!c->pdl || c->plain_next) {
+    c->plain_next = false;
+    kernel<<<grid, block, smem, c->launch_stream>>>(ra);
+    return;
+  }
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof cfg);
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = c->launch_stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, kernel, ra);
+}
+#endif
+
+// The tile kernel of shader S for the target's format.  Runs: the kind is drawn under depth test with
+// failing-sample bitmaps, so a batch that has them takes the depth-run variant (RGBA8 targets only).
+template <class S, bool Runs>
+static void launch_tiles(wrcu_ctx* c, const RasterArgs& ra, int grid, bool depth_runs) {
+#ifndef WRCU_HOSTEMU
+  if constexpr (Runs) {
+    if (depth_runs && ra.tgt.fmt == WRCU_FMT_RGBA8) {
+      auto k_runs = wr_raster<S, WRCU_FMT_RGBA8, true>;
+      WR_LAUNCH_CHAIN(k_runs, grid, WRCU_THREADS, ra);
+      return;
+    }
+  }
+#endif
+  auto k_rgba = wr_raster<S, WRCU_FMT_RGBA8>;
+  auto k_r8 = wr_raster<S, WRCU_FMT_R8>;
+  if (ra.tgt.fmt == WRCU_FMT_RGBA8) WR_LAUNCH_CHAIN(k_rgba, grid, WRCU_THREADS, ra);
+  else WR_LAUNCH_CHAIN(k_r8, grid, WRCU_THREADS, ra);
+}
+typedef void (*TileLaunch)(wrcu_ctx* c, const RasterArgs& ra, int grid, bool depth_runs);
+
+// Depth runs matter to kinds whose shading depends on the position inside a span (AA ramps, span shader vs
+// fragment tail, interpolated varyings).  Plain solids with blending off never do (their AA / mask flags are
+// dropped, setup_common.cuh wr_emit_quad).
+enum { RUNS_NEVER, RUNS_ALWAYS, RUNS_IF_BLENDING };
+
+// What the draw path knows about each program kind, one row per WRCU_KIND_* (row 0: no kind).  Rules that
+// depend on more than the kind are code where the row is read (draw_batch_impl, launch_raster).
+struct KindDesc {
+  const char* program;    // shader name (wrcu_program_from_name)
+  const char* record;     // instance record ...
+  unsigned min_stride;    //   ... and its size: the least instance stride
+  unsigned samplers;      // bit i: sColor<i> must be bound
+  int color0_fmt;         // the format sColor0 must have, 0: any
+  int runs;               // RUNS_*: failing-sample bitmaps for depth-tested batches
+  bool persp;             // the fragment stage carries the draw_perspective (per-sample 1/w) path
+  bool fast;              // may emit CMD_CONST_COLOR: the solid / fold kernels may draw the batch
+  bool strip;             // may take strip mode (raster.cuh WrRowReuse)
+  TileLaunch tiles;
+  uint32_t alt_feature;   // with this feature: alt_tiles and alt_persp instead of tiles and persp
+  TileLaunch alt_tiles;
+  bool alt_persp;
+};
+static const KindDesc kinds[] = {
+    {},
+    {"ps_quad_textured", "PrimitiveInstanceData", 16, 0, 0, RUNS_ALWAYS, true, true, false, launch_tiles<QuadShader, true>},
+    {"ps_quad_mask", "MaskInstance", 32, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<QuadMaskShader, false>},
+    {"brush_solid", "PrimitiveInstanceData", 16, 0, 0, RUNS_IF_BLENDING, true, true, false, launch_tiles<QuadShader, true>},
+    {"brush_image", "PrimitiveInstanceData", 16, 1, 0, RUNS_ALWAYS, true, false, false, launch_tiles<ImageShader, true>,
+     WRCU_FEAT_REPETITION, launch_tiles<ImageRepeatShader, true>, false},
+    {"brush_linear_gradient", "PrimitiveInstanceData", 16, 0, 0, RUNS_ALWAYS, false, false, true, launch_tiles<GradientShader, true>},
+    {"brush_blend", "PrimitiveInstanceData", 16, 1, 0, RUNS_ALWAYS, true, false, false, launch_tiles<BlendShader, true>},
+    {"brush_mix_blend", "PrimitiveInstanceData", 16, 3, 0, RUNS_ALWAYS, true, false, false, launch_tiles<MixBlendShader, true>},
+    {"brush_opacity", "PrimitiveInstanceData", 16, 1, 0, RUNS_ALWAYS, true, false, false, launch_tiles<OpacityShader, true>},
+    {"ps_text_run", "PrimitiveInstanceData", 16, 1, 0, RUNS_ALWAYS, false, false, false, launch_tiles<TextShader, true>},
+    {"cs_clip_rectangle", "ClipMaskInstanceRect", 200, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<ClipRectShader, false>},
+    {"cs_clip_box_shadow", "ClipMaskInstanceBoxShadow", 84, 1, WRCU_FMT_R8, RUNS_NEVER, false, false, false,
+     launch_tiles<BoxShadowShader, false>},
+    {"composite", "CompositeInstance", 120, 1, 0, RUNS_NEVER, false, false, true, launch_tiles<CompositeShader, false>,
+     WRCU_FEAT_YUV, launch_tiles<CompositeYuvShader, false>, false},
+    {"ps_clear", "ClearInstance", 32, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<QuadShader, true>},
+    {"cs_blur", "BlurInstance", 24, 1, 0, RUNS_NEVER, false, false, false, launch_tiles<BlurShader, false>},
+    {"cs_scale", "ScalingInstance", 36, 1, 0, RUNS_NEVER, false, false, false, launch_tiles<ScaleShader, false>},
+    {"cs_fast_linear_gradient", "FastLinearGradientInstance", 52, 0, 0, RUNS_NEVER, false, false, false,
+     launch_tiles<FastLinearShader, false>},
+    {"cs_linear_gradient", "LinearGradientInstance", 48, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<GradientShader, false>},
+    {"cs_radial_gradient", "RadialGradientInstance", 52, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<RadialShader, false>},
+    {"cs_conic_gradient", "ConicGradientInstance", 52, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<ConicShader, false>},
+    {"cs_line_decoration", "LineDecorationJob", 36, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<LineDecorationShader, false>},
+    {"cs_border_solid", "BorderInstance", 108, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<BorderSolidShader, false>},
+    {"cs_border_segment", "BorderInstance", 108, 0, 0, RUNS_NEVER, false, false, false, launch_tiles<BorderSegmentShader, false>},
+    {"ps_quad_radial_gradient", "PrimitiveInstanceData", 16, 0, 0, RUNS_ALWAYS, false, false, false, launch_tiles<RadialShader, true>},
+    {"ps_quad_conic_gradient", "PrimitiveInstanceData", 16, 0, 0, RUNS_ALWAYS, false, false, false, launch_tiles<QuadConicShader, true>},
+    {"brush_yuv_image", "PrimitiveInstanceData", 16, 1, 0, RUNS_ALWAYS, false, false, true, launch_tiles<CompositeYuvShader, true>},
+    {"ps_split_composite", "PrimitiveInstanceData", 16, 1, WRCU_FMT_RGBA8, RUNS_ALWAYS, true, false, false, launch_tiles<ImageShader, true>},
+};
+static const int N_KINDS = (int)(sizeof kinds / sizeof kinds[0]);
+
 static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_draw_state* st,
                            const void* instances, size_t stride, int n, const wrcu_tex* textures);
 
@@ -1465,7 +1569,6 @@ extern "C" int wrcu_draw_composite_tiles(wrcu_ctx* c, uint32_t features, const w
   return draw_batch_impl(c, WRCU_KIND_COMPOSITE, features, st, instances, stride, n, textures);
 }
 
-#define WR_COPY_MAX_CMDS_HOST 128  // = WR_COPY_MAX_CMDS (shader_composite.cuh): the copy kernel's staged command list
 static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_draw_state* st,
                            const void* instances, size_t stride, int n, const wrcu_tex* textures) {
   if (!st || !instances || n < 0 || stride == 0)
@@ -1521,6 +1624,23 @@ static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_
 
   if (T.cx1 <= T.cx0 || T.cy1 <= T.cy0) return WRCU_OK;  // scissor misses the target: SWGL draws nothing
 
+  if (kind <= 0 || kind >= N_KINDS) return wrcu_fail(c, WRCU_ERR_UNSUPPORTED, "draw_batch: kind %d not implemented", kind);
+  const KindDesc& K = kinds[kind];
+  if (stride < K.min_stride)
+    return wrcu_fail(c, WRCU_ERR_INVALID, "%s: %s stride %zu < %u", K.program, K.record, stride, K.min_stride);
+  // SWGL builds no dual-source variant of brush_image
+  if (kind == WRCU_KIND_BRUSH_IMAGE && (features & WRCU_FEAT_DUAL_SOURCE_BLENDING))
+    return wrcu_fail(c, WRCU_ERR_UNSUPPORTED, "brush_image DUAL_SOURCE_BLENDING variant not built (SWGL does not build it either)");
+  // a tile list samples one texture per instance; sColor0 is the first instance's
+  const TexView color[3] = {tex_view(c, textures ? textures[0] : st->color[0]), tex_view(c, st->color[1]), tex_view(c, st->color[2])};
+  for (int i = 0; i < 3; i++)
+    if ((K.samplers >> i & 1) && !color[i].ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "%s without sColor%d", K.program, i);
+  if (K.color0_fmt && color[0].fmt != K.color0_fmt)
+    return wrcu_fail(c, WRCU_ERR_INVALID, "%s needs an %s surface in sColor0", K.program, K.color0_fmt == WRCU_FMT_R8 ? "R8" : "RGBA8");
+  // cs_blur is built once per output format, and the feature names which one the batch draws with
+  if (kind == WRCU_KIND_BLUR && !(features & (WRCU_FEAT_ALPHA_TARGET | WRCU_FEAT_COLOR_TARGET)))
+    return wrcu_fail(c, WRCU_ERR_INVALID, "cs_blur needs ALPHA_TARGET or COLOR_TARGET");
+
   SetupArgs sa;
   memset(&sa, 0, sizeof sa);
   sa.tgt = T;
@@ -1530,42 +1650,26 @@ static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_
   // (hot / cold / info / pool pointers are assigned when the submission is flushed)
   sa.err_counter = c->dev_err;
   sa.blend_enabled = st->blend != WRCU_BLEND_NONE;
+  sa.features = features;
+  sa.kind = kind;
 #ifndef WRCU_HOSTEMU
-  {
-    // Depth runs matter to kinds whose shading depends on the position inside a span (AA ramps, span
-    // shader vs fragment tail, interpolated varyings).  Plain solids with blending off never do (their
-    // AA / mask flags are dropped, setup_common.cuh wr_emit_quad).
-    bool kind_runs = false;
-    switch (kind) {
-      case WRCU_KIND_BRUSH_SOLID: kind_runs = st->blend != WRCU_BLEND_NONE; break;
-      case WRCU_KIND_QUAD_TEXTURED: case WRCU_KIND_BRUSH_IMAGE: case WRCU_KIND_BRUSH_LINEAR_GRADIENT:
-      case WRCU_KIND_BRUSH_BLEND: case WRCU_KIND_BRUSH_MIX_BLEND: case WRCU_KIND_BRUSH_OPACITY: case WRCU_KIND_TEXT_RUN:
-      case WRCU_KIND_BRUSH_YUV_IMAGE: case WRCU_KIND_QUAD_RADIAL_GRADIENT: case WRCU_KIND_QUAD_CONIC_GRADIENT:
-      case WRCU_KIND_SPLIT_COMPOSITE:
-        kind_runs = true; break;
-      default: break;
+  if (T.depth && (K.runs == RUNS_ALWAYS || (K.runs == RUNS_IF_BLENDING && st->blend != WRCU_BLEND_NONE))) {
+    if (!c->fail_pool) {
+      c->fail_cap = 16 << 20;  // 64 MiB of bitmaps per batch; commands beyond it keep span-relative phase
+      if (cudaMalloc((void**)&c->fail_pool, (size_t)c->fail_cap * 4) != cudaSuccess) {
+        c->fail_pool = nullptr;
+        c->fail_cap = 0;
+        cudaGetLastError();
+      }
     }
-    if (kind_runs && T.depth) {
-      if (!c->fail_pool) {
-        c->fail_cap = 16 << 20;  // 64 MiB of bitmaps per batch; commands beyond it keep span-relative phase
-        if (cudaMalloc((void**)&c->fail_pool, (size_t)c->fail_cap * 4) != cudaSuccess) {
-          c->fail_pool = nullptr;
-          c->fail_cap = 0;
-          cudaGetLastError();
-        }
-      }
-      if (c->fail_pool) {
-        sa.depth_runs = 1;
-        sa.fail_cap = c->fail_cap;
-      }
+    if (c->fail_pool) {
+      sa.depth_runs = 1;
+      sa.fail_cap = c->fail_cap;
     }
   }
 #endif
-  // draw_perspective (w differs between an instance's vertices): the kinds whose fragment stage carries the
-  // per-sample 1/w path; the solid colour case of ps_quad_textured shares brush_solid's shader
-  sa.persp_ok = kind == WRCU_KIND_BRUSH_SOLID || kind == WRCU_KIND_SPLIT_COMPOSITE || kind == WRCU_KIND_QUAD_TEXTURED ||
-                kind == WRCU_KIND_BRUSH_OPACITY || kind == WRCU_KIND_BRUSH_BLEND || kind == WRCU_KIND_BRUSH_MIX_BLEND ||
-                (kind == WRCU_KIND_BRUSH_IMAGE && !(features & WRCU_FEAT_REPETITION));
+  // draw_perspective: w differs between an instance's vertices
+  sa.persp_ok = (features & K.alt_feature) ? K.alt_persp : K.persp;
   // copy class (shader_composite.cuh): 1 = 1:1 tile copies and solid fills, 2 = fills only (the clear tile's dest-out)
   sa.copy_ok = T.depth ? 0 : (st->blend == WRCU_BLEND_NONE || st->blend == WRCU_BLEND_PREMULTIPLIED_ALPHA) ? 1
                              : st->blend == WRCU_BLEND_PREMULTIPLIED_DEST_OUT ? 2 : 0;
@@ -1573,7 +1677,7 @@ static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_
     // The copy kernel moves boxes of different instances concurrently: a batch whose instances overlap keeps
     // the ordered tile kernel.  Picture-cache tiles never overlap; checked here on the host copies of the
     // CompositeInstance rects (device rect ∩ clip rect, rounded outwards), n is a tile list's length.
-    if (n > WR_COPY_MAX_CMDS_HOST || stride < 32) sa.copy_ok = 0;
+    if (n > WR_COPY_MAX_CMDS) sa.copy_ok = 0;
     else {
       std::vector<float> bb((size_t)n * 4);
       for (int i = 0; i < n; i++) {
@@ -1590,10 +1694,9 @@ static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_
       }
     }
   }
-  sa.color0 = tex_view(c, st->color[0]);
-  sa.color1 = tex_view(c, st->color[1]);
-  sa.color2 = tex_view(c, st->color[2]);
-  if (textures) sa.color0 = tex_view(c, textures[0]);  // (sa.tex_list: resolved from views_off at flush)
+  sa.color0 = color[0];  // (sa.tex_list: resolved from views_off at flush)
+  sa.color1 = color[1];
+  sa.color2 = color[2];
   size_t bin_need = 0;
   // Bitmask bins for batches with many instances: the per-tile command scan of the raster
   // kernel costs tiles x n hot records of L2 traffic; with bins it reads n/32 words per tile.
@@ -1620,141 +1723,6 @@ static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_
     sblocks = (n * 32 + 127) / 128;
   }
 #endif
-  switch (kind) {
-    case WRCU_KIND_QUAD_TEXTURED:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "quad instance stride < 16");
-      /* set-up: wr_setup_quad_textured, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_SOLID:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      /* set-up: wr_setup_brush_solid, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_IMAGE:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (features & WRCU_FEAT_DUAL_SOURCE_BLENDING)
-        return wrcu_fail(c, WRCU_ERR_UNSUPPORTED, "brush_image DUAL_SOURCE_BLENDING variant not built (SWGL does not build it either)");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "brush_image without sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_brush_image, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_LINEAR_GRADIENT:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      sa.features = features;
-      /* set-up: wr_setup_brush_linear_gradient, run by flush_pending */;
-      break;
-    case WRCU_KIND_TEXT_RUN:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "ps_text_run without sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_text_run, run by flush_pending */;
-      break;
-    case WRCU_KIND_QUAD_MASK:
-      if (stride < 32) return wrcu_fail(c, WRCU_ERR_INVALID, "MaskInstance stride < 32");
-      sa.features = features;
-      /* set-up: wr_setup_quad_mask, run by flush_pending */;
-      break;
-    case WRCU_KIND_CLIP_RECTANGLE:
-      if (stride < 200) return wrcu_fail(c, WRCU_ERR_INVALID, "ClipMaskInstanceRect stride < 200");
-      sa.features = features;
-      /* set-up: wr_setup_clip_rectangle, run by flush_pending */;
-      break;
-    case WRCU_KIND_SCALE:
-      if (stride < 36) return wrcu_fail(c, WRCU_ERR_INVALID, "ScalingInstance stride < 36");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "cs_scale without sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_scale, run by flush_pending */;
-      break;
-    case WRCU_KIND_QUAD_RADIAL_GRADIENT:
-    case WRCU_KIND_QUAD_CONIC_GRADIENT:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      sa.features = features;
-      sa.kind = kind;
-      /* set-up: wr_setup_quad_gradient, run by flush_pending */;
-      break;
-    case WRCU_KIND_LINE_DECORATION:
-      if (stride < 36) return wrcu_fail(c, WRCU_ERR_INVALID, "LineDecorationJob stride < 36");
-      sa.features = features;
-      /* set-up: wr_setup_line_decoration, run by flush_pending */;
-      break;
-    case WRCU_KIND_BORDER_SOLID:
-    case WRCU_KIND_BORDER_SEGMENT:
-      if (stride < 108) return wrcu_fail(c, WRCU_ERR_INVALID, "BorderInstance stride < 108");
-      sa.features = features;
-      sa.kind = kind;
-      /* set-up: wr_setup_border, run by flush_pending */;
-      break;
-    case WRCU_KIND_FAST_LINEAR_GRADIENT:
-    case WRCU_KIND_LINEAR_GRADIENT:
-    case WRCU_KIND_RADIAL_GRADIENT:
-    case WRCU_KIND_CONIC_GRADIENT:
-      if (stride < (kind == WRCU_KIND_LINEAR_GRADIENT ? 48u : 52u))
-        return wrcu_fail(c, WRCU_ERR_INVALID, "gradient task instance stride too small");
-      sa.features = features;
-      sa.kind = kind;
-      /* set-up: wr_setup_cs_gradient, run by flush_pending */;
-      break;
-    case WRCU_KIND_BLUR:
-      if (stride < 24) return wrcu_fail(c, WRCU_ERR_INVALID, "BlurInstance stride < 24");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "cs_blur without sColor0");
-      if (!(features & (WRCU_FEAT_ALPHA_TARGET | WRCU_FEAT_COLOR_TARGET)))
-        return wrcu_fail(c, WRCU_ERR_INVALID, "cs_blur needs ALPHA_TARGET or COLOR_TARGET");
-      sa.features = features;
-      /* set-up: wr_setup_blur, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_MIX_BLEND:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (!sa.color0.ptr || !sa.color1.ptr)
-        return wrcu_fail(c, WRCU_ERR_INVALID, "brush_mix_blend needs sColor0 (backdrop) and sColor1 (source)");
-      sa.features = features;
-      /* set-up: wr_setup_brush_mix_blend, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_BLEND:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "brush_blend without sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_brush_blend, run by flush_pending */;
-      break;
-    case WRCU_KIND_CLEAR:
-      if (stride < 32) return wrcu_fail(c, WRCU_ERR_INVALID, "ClearInstance stride < 32");
-      /* set-up: wr_setup_clear, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_OPACITY:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "brush_opacity without sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_brush_opacity, run by flush_pending */;
-      break;
-    case WRCU_KIND_SPLIT_COMPOSITE:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (!sa.color0.ptr || sa.color0.fmt != WRCU_FMT_RGBA8)
-        return wrcu_fail(c, WRCU_ERR_INVALID, "ps_split_composite needs an RGBA8 surface in sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_split_composite, run by flush_pending */;
-      break;
-    case WRCU_KIND_BRUSH_YUV_IMAGE:
-      if (stride < 16) return wrcu_fail(c, WRCU_ERR_INVALID, "prim instance stride < 16");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "brush_yuv_image without sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_brush_yuv_image, run by flush_pending */;
-      break;
-    case WRCU_KIND_COMPOSITE:
-      if (stride < 120) return wrcu_fail(c, WRCU_ERR_INVALID, "CompositeInstance stride < 120");
-      if (!sa.color0.ptr) return wrcu_fail(c, WRCU_ERR_INVALID, "composite without sColor0");
-      sa.features = features;
-      if (features & WRCU_FEAT_YUV) /* set-up: wr_setup_composite_yuv, run by flush_pending */;
-      else /* set-up: wr_setup_composite, run by flush_pending */;
-      break;
-    case WRCU_KIND_CLIP_BOX_SHADOW:
-      if (stride < 84) return wrcu_fail(c, WRCU_ERR_INVALID, "ClipMaskInstanceBoxShadow stride < 84");
-      if (!sa.color0.ptr || sa.color0.fmt != WRCU_FMT_R8)
-        return wrcu_fail(c, WRCU_ERR_INVALID, "cs_clip_box_shadow needs an R8 shadow mask in sColor0");
-      sa.features = features;
-      /* set-up: wr_setup_clip_box_shadow, run by flush_pending */;
-      break;
-    default:
-      return wrcu_fail(c, WRCU_ERR_UNSUPPORTED, "draw_batch: kind %d not implemented", kind);
-  }
-
   RasterArgs ra;
   memset(&ra, 0, sizeof ra);
   ra.tgt = T;
@@ -1796,38 +1764,12 @@ static int draw_batch_impl(wrcu_ctx* c, int kind, uint32_t features, const wrcu_
   return WRCU_OK;
 }
 
-#ifndef WRCU_HOSTEMU
-// A raster-class launch with programmatic stream serialization (see raster.cuh wr_pdl_wait); the ordinary
-// launch when the context has it switched off (WRCU_PDL=0).
-template <typename K>
-static void wr_launch_chain(wrcu_ctx* c, K kernel, unsigned grid, unsigned block, size_t smem, const RasterArgs& ra) {
-  // (a launch that directly follows an event wait in its stream is an ordinary one: the programmatic edge is
-  // between two kernels, and nothing is gained by leaving it to the driver what an event wait in between means)
-  if (!c->pdl || c->plain_next) {
-    c->plain_next = false;
-    kernel<<<grid, block, smem, c->launch_stream>>>(ra);
-    return;
-  }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof cfg);
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(block);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = c->launch_stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  cudaLaunchKernelEx(&cfg, kernel, ra);
-}
-#endif
-
 // The raster launches of one queued batch (its set-up has run): depth-run prepass, then the kernel(s) of its kind.
 static int launch_raster(wrcu_ctx* c, PendingOp& op) {
   RasterArgs& ra = op.ra;
   const TargetDev& T = ra.tgt;
   const int kind = op.kind, n = op.n;
+  const KindDesc& K = kinds[kind];
   const uint32_t features = op.features;
   dim3 grid(op.grid_x, op.grid_y);
   // Device-side dispatch: the setup kernel decides whether the whole batch is
@@ -1847,9 +1789,7 @@ static int launch_raster(wrcu_ctx* c, PendingOp& op) {
   }
 #endif
   if (c->profile) WRCU_CUDA(c, cudaEventRecord(c->p0, c->launch_stream));
-  bool fast_ok = T.fmt == WRCU_FMT_RGBA8 && op.blend == WRCU_BLEND_PREMULTIPLIED_ALPHA &&
-                 ra.depth_mode == WRCU_DEPTH_OFF &&
-                 (kind == WRCU_KIND_QUAD_TEXTURED || kind == WRCU_KIND_BRUSH_SOLID);  // the only kinds that emit CMD_CONST_COLOR
+  bool fast_ok = T.fmt == WRCU_FMT_RGBA8 && op.blend == WRCU_BLEND_PREMULTIPLIED_ALPHA && ra.depth_mode == WRCU_DEPTH_OFF && K.fast;
   ra.fast_eligible = fast_ok ? 1 : 0;
   ra.fold = nullptr;
   if (fast_ok) {
@@ -1915,105 +1855,46 @@ static int launch_raster(wrcu_ctx* c, PendingOp& op) {
   // strip mode (raster.cuh WrRowReuse): few commands on a wide target — work items become runs of adjacent tiles,
   // as long as there are still about two items per resident CTA
   ra.strip_seg = 0;
-  if (c->strip && n <= 16 && (kind == WRCU_KIND_COMPOSITE || kind == WRCU_KIND_BRUSH_YUV_IMAGE || kind == WRCU_KIND_BRUSH_LINEAR_GRADIENT)) {
+  if (c->strip && n <= 16 && K.strip) {
     int seg = 10;
     while (seg > 1 && (((int)grid.x + seg - 1) / seg) * (int)grid.y < 2 * max_ctas) seg--;
     if (seg > 1) ra.strip_seg = seg;
   }
-#define LAUNCH_RASTER(S)                                                         \
-  do {                                                                           \
-    auto k_rgba = wr_raster<S, WRCU_FMT_RGBA8>;                                   \
-    auto k_r8 = wr_raster<S, WRCU_FMT_R8>;                                        \
-    if (T.fmt == WRCU_FMT_RGBA8)                                                 \
-      WR_LAUNCH_CHAIN(k_rgba, pgrid, WRCU_THREADS, ra);                          \
-    else                                                                         \
-      WR_LAUNCH_CHAIN(k_r8, pgrid, WRCU_THREADS, ra);                            \
-  } while (0)
-  // kinds drawn under depth test: the depth-run variant when this batch has failing-sample bitmaps
-#ifdef WRCU_HOSTEMU
-#define LAUNCH_RASTER_RUNS(S) LAUNCH_RASTER(S)
-#else
-#define LAUNCH_RASTER_RUNS(S)                                                    \
-  do {                                                                           \
-    if (op.sa.depth_runs && T.fmt == WRCU_FMT_RGBA8) {                              \
-      auto k_runs = wr_raster<S, WRCU_FMT_RGBA8, true>;                           \
-      WR_LAUNCH_CHAIN(k_runs, pgrid, WRCU_THREADS, ra);                          \
-    } else LAUNCH_RASTER(S);                                                     \
-  } while (0)
-#endif
-  switch (kind) {
-    case WRCU_KIND_CLIP_RECTANGLE: LAUNCH_RASTER(ClipRectShader); break;
-    case WRCU_KIND_QUAD_MASK: LAUNCH_RASTER(QuadMaskShader); break;
-    case WRCU_KIND_BRUSH_IMAGE:
-      if (features & WRCU_FEAT_REPETITION) LAUNCH_RASTER_RUNS(ImageRepeatShader);
-      else LAUNCH_RASTER_RUNS(ImageShader);
-      break;
-    case WRCU_KIND_TEXT_RUN:
 #ifndef WRCU_HOSTEMU
-      // glyph-major first (a warp per glyph, shader_text.cuh); the tile kernel then draws what it flagged CMD_ORDERED
-      if (c->glyph_major && T.fmt == WRCU_FMT_RGBA8 && n >= 8 &&
-          (ra.depth_mode == WRCU_DEPTH_OFF || (ra.depth_mode == WRCU_DEPTH_TEST && op.sa.depth_runs))) {
-        ra.glyph_major = 1;
-        auto k_glyphs = wr_raster_glyphs<WRCU_FMT_RGBA8>;
-        const int per_cta = WR_GLYPH_THREADS / 32;
-        int ggrid = (n + per_cta - 1) / per_cta;           // persistent warps taking glyphs by ticket
-        if (ggrid > c->sm_count * c->glyph_ctas) ggrid = c->sm_count * c->glyph_ctas;
-        wr_launch_chain(c, k_glyphs, (unsigned)ggrid, WR_GLYPH_THREADS, 0, ra);
-        c->stats.kernel_launches++;
-        ra.pdl_early = 0;  // the tile kernel reads what the glyph kernel wrote (flags, BatchInfo::n_ordered)
-      }
-#endif
-      LAUNCH_RASTER_RUNS(TextShader);
-      break;
-    case WRCU_KIND_BRUSH_LINEAR_GRADIENT: LAUNCH_RASTER_RUNS(GradientShader); break;
-    case WRCU_KIND_CLIP_BOX_SHADOW: LAUNCH_RASTER(BoxShadowShader); break;
-    case WRCU_KIND_BRUSH_YUV_IMAGE: LAUNCH_RASTER_RUNS(CompositeYuvShader); break;
-    case WRCU_KIND_SPLIT_COMPOSITE: LAUNCH_RASTER_RUNS(ImageShader); break;
-    case WRCU_KIND_COMPOSITE:
-      if (features & WRCU_FEAT_YUV) {
-#ifndef WRCU_HOSTEMU
-        if (c->yuv_wide && T.fmt == WRCU_FMT_RGBA8) { auto k_w = wr_raster<CompositeYuvShaderWide, WRCU_FMT_RGBA8>; WR_LAUNCH_CHAIN(k_w, pgrid, WRCU_THREADS, ra); break; }
-#endif
-        LAUNCH_RASTER(CompositeYuvShader);
-        break;
-      }
-#ifndef WRCU_HOSTEMU
-      if (c->tmaps_dev && T.tmap_id && op.sa.copy_ok) {
-        // copy-class tile lists (decided on the device, BatchInfo::all_copy) go through the copy engine;
-        // whichever of the two kernels is not in charge returns at once
-        const size_t smem0 = (size_t)WR_TMA_STAGES * WR_TMA_BOX_BYTES, smem1 = (size_t)WR_TMA_BLEND_STAGES * 2 * WR_TMA_BOX_BYTES;
-        if (!c->copy_attr_set) {
-          WRCU_CUDA(c, cudaFuncSetAttribute(wr_composite_copy<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem0));
-          WRCU_CUDA(c, cudaFuncSetAttribute(wr_composite_copy<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-          c->copy_attr_set = true;
-        }
-        ra.copy_eligible = 1;
-        if (op.blend == WRCU_BLEND_NONE) wr_launch_chain(c, wr_composite_copy<0>, (unsigned)c->sm_count * 3, WR_TMA_THREADS, smem0, ra);
-        else if (op.blend == WRCU_BLEND_PREMULTIPLIED_ALPHA) wr_launch_chain(c, wr_composite_copy<1>, (unsigned)c->sm_count * 2, WR_TMA_THREADS, smem1, ra);
-        else wr_launch_chain(c, wr_composite_copy<2>, (unsigned)c->sm_count * 2, WR_TMA_THREADS, 0, ra);
-        c->stats.kernel_launches++;
-      }
-#endif
-      LAUNCH_RASTER(CompositeShader);
-      break;
-    case WRCU_KIND_BRUSH_OPACITY: LAUNCH_RASTER_RUNS(OpacityShader); break;
-    case WRCU_KIND_BRUSH_BLEND: LAUNCH_RASTER_RUNS(BlendShader); break;
-    case WRCU_KIND_BRUSH_MIX_BLEND: LAUNCH_RASTER_RUNS(MixBlendShader); break;
-    case WRCU_KIND_BLUR: LAUNCH_RASTER(BlurShader); break;
-    case WRCU_KIND_SCALE: LAUNCH_RASTER(ScaleShader); break;
-    case WRCU_KIND_FAST_LINEAR_GRADIENT: LAUNCH_RASTER(FastLinearShader); break;
-    case WRCU_KIND_LINEAR_GRADIENT: LAUNCH_RASTER(GradientShader); break;
-    case WRCU_KIND_RADIAL_GRADIENT: LAUNCH_RASTER(RadialShader); break;
-    case WRCU_KIND_CONIC_GRADIENT: LAUNCH_RASTER(ConicShader); break;
-    case WRCU_KIND_QUAD_RADIAL_GRADIENT: LAUNCH_RASTER_RUNS(RadialShader); break;
-    case WRCU_KIND_QUAD_CONIC_GRADIENT: LAUNCH_RASTER_RUNS(QuadConicShader); break;
-    case WRCU_KIND_LINE_DECORATION: LAUNCH_RASTER(LineDecorationShader); break;
-    case WRCU_KIND_BORDER_SOLID: LAUNCH_RASTER(BorderSolidShader); break;
-    case WRCU_KIND_BORDER_SEGMENT: LAUNCH_RASTER(BorderSegmentShader); break;
-    default: LAUNCH_RASTER_RUNS(QuadShader); break;
+  // glyph-major first (a warp per glyph, shader_text.cuh); the tile kernel then draws what it flagged CMD_ORDERED
+  if (kind == WRCU_KIND_TEXT_RUN && c->glyph_major && T.fmt == WRCU_FMT_RGBA8 && n >= 8 &&
+      (ra.depth_mode == WRCU_DEPTH_OFF || (ra.depth_mode == WRCU_DEPTH_TEST && op.sa.depth_runs))) {
+    ra.glyph_major = 1;
+    auto k_glyphs = wr_raster_glyphs<WRCU_FMT_RGBA8>;
+    const int per_cta = WR_GLYPH_THREADS / 32;
+    int ggrid = (n + per_cta - 1) / per_cta;           // persistent warps taking glyphs by ticket
+    if (ggrid > c->sm_count * c->glyph_ctas) ggrid = c->sm_count * c->glyph_ctas;
+    wr_launch_chain(c, k_glyphs, (unsigned)ggrid, WR_GLYPH_THREADS, 0, ra);
+    c->stats.kernel_launches++;
+    ra.pdl_early = 0;  // the tile kernel reads what the glyph kernel wrote (flags, BatchInfo::n_ordered)
   }
-#undef LAUNCH_RASTER
-#undef LAUNCH_RASTER_RUNS
+  if (kind == WRCU_KIND_COMPOSITE && !(features & WRCU_FEAT_YUV) && c->tmaps_dev && T.tmap_id && op.sa.copy_ok) {
+    // copy-class tile lists (decided on the device, BatchInfo::all_copy) go through the copy engine;
+    // whichever of the two kernels is not in charge returns at once
+    const size_t smem0 = (size_t)WR_TMA_STAGES * WR_TMA_BOX_BYTES, smem1 = (size_t)WR_TMA_BLEND_STAGES * 2 * WR_TMA_BOX_BYTES;
+    if (!c->copy_attr_set) {
+      WRCU_CUDA(c, cudaFuncSetAttribute(wr_composite_copy<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem0));
+      WRCU_CUDA(c, cudaFuncSetAttribute(wr_composite_copy<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+      c->copy_attr_set = true;
+    }
+    ra.copy_eligible = 1;
+    if (op.blend == WRCU_BLEND_NONE) wr_launch_chain(c, wr_composite_copy<0>, (unsigned)c->sm_count * 3, WR_TMA_THREADS, smem0, ra);
+    else if (op.blend == WRCU_BLEND_PREMULTIPLIED_ALPHA) wr_launch_chain(c, wr_composite_copy<1>, (unsigned)c->sm_count * 2, WR_TMA_THREADS, smem1, ra);
+    else wr_launch_chain(c, wr_composite_copy<2>, (unsigned)c->sm_count * 2, WR_TMA_THREADS, 0, ra);
+    c->stats.kernel_launches++;
+  }
+  if (kind == WRCU_KIND_COMPOSITE && (features & WRCU_FEAT_YUV) && c->yuv_wide && T.fmt == WRCU_FMT_RGBA8) {
+    // WRCU_YUV_WIDE=1: composite YUV through its one-CTA-per-SM build, for measuring against the default
+    auto k_w = wr_raster<CompositeYuvShaderWide, WRCU_FMT_RGBA8>;
+    WR_LAUNCH_CHAIN(k_w, pgrid, WRCU_THREADS, ra);
+  } else
+#endif
+    ((features & K.alt_feature) ? K.alt_tiles : K.tiles)(c, ra, pgrid, op.sa.depth_runs);
   c->stats.kernel_launches++;
   if (c->profile) {
     WRCU_CUDA(c, cudaEventRecord(c->p1, c->launch_stream));
@@ -2032,24 +1913,9 @@ struct __align__(16) SetupJob {
   int first_block;   // of this job in the launch
   int pad;
 };
-#ifndef WRCU_HOSTEMU
-__global__ void __launch_bounds__(128) wr_setup_multi(const SetupJob* jobs, const int* block_job, BatchInfo* reset, int n_reset,
-                                                      int* reset_ctr) {
-  __shared__ SetupJob sj;
-  if (blockIdx.x == 0) {  // re-arm the records the NEXT submission will use (the other half of the ring)
-    for (int i = threadIdx.x; i < n_reset; i += blockDim.x) wr_reset_batch_info(reset + i);
-    if (threadIdx.x < 2) reset_ctr[threadIdx.x] = 0;
-  }
-  const int j = __ldg(block_job + blockIdx.x);
-  {
-    const uint4* src = (const uint4*)(jobs + j);
-    uint4* dst = (uint4*)&sj;
-    for (int i = threadIdx.x; i < (int)(sizeof(SetupJob) / 16); i += blockDim.x) dst[i] = __ldg(src + i);
-  }
-  __syncthreads();
-  const SetupArgs& a = sj.a;
-  const int idx = ((int)blockIdx.x - sj.first_block) * (int)blockDim.x + (int)threadIdx.x;
-  switch (sj.kind) {
+// The set-up of thread idx of one batch (on the host: of the whole batch).
+WRD void wr_setup_batch(int kind, uint32_t features, const SetupArgs& a, int idx) {
+  switch (kind) {
     case WRCU_KIND_QUAD_TEXTURED: wr_setup_quad_textured_block(a, idx); break;
     case WRCU_KIND_QUAD_MASK: wr_setup_quad_mask_block(a, idx); break;
     case WRCU_KIND_BRUSH_SOLID: wr_setup_brush_solid_block(a, idx); break;
@@ -2062,7 +1928,7 @@ __global__ void __launch_bounds__(128) wr_setup_multi(const SetupJob* jobs, cons
     case WRCU_KIND_CLIP_RECTANGLE: wr_setup_clip_rectangle_block(a, idx); break;
     case WRCU_KIND_CLIP_BOX_SHADOW: wr_setup_clip_box_shadow_block(a, idx); break;
     case WRCU_KIND_COMPOSITE:
-      if (sj.features & WRCU_FEAT_YUV) wr_setup_composite_yuv_block(a, idx);
+      if (features & WRCU_FEAT_YUV) wr_setup_composite_yuv_block(a, idx);
       else wr_setup_composite_block(a, idx);
       break;
     case WRCU_KIND_CLEAR: wr_setup_clear_block(a, idx); break;
@@ -2078,36 +1944,22 @@ __global__ void __launch_bounds__(128) wr_setup_multi(const SetupJob* jobs, cons
     default: break;
   }
 }
-#else
-static void setup_host(int kind, uint32_t features, const SetupArgs& a) {
-  switch (kind) {
-    case WRCU_KIND_QUAD_TEXTURED: wr_setup_quad_textured(a); break;
-    case WRCU_KIND_QUAD_MASK: wr_setup_quad_mask(a); break;
-    case WRCU_KIND_BRUSH_SOLID: wr_setup_brush_solid(a); break;
-    case WRCU_KIND_BRUSH_IMAGE: wr_setup_brush_image(a); break;
-    case WRCU_KIND_BRUSH_LINEAR_GRADIENT: wr_setup_brush_linear_gradient(a); break;
-    case WRCU_KIND_BRUSH_BLEND: wr_setup_brush_blend(a); break;
-    case WRCU_KIND_BRUSH_MIX_BLEND: wr_setup_brush_mix_blend(a); break;
-    case WRCU_KIND_BRUSH_OPACITY: wr_setup_brush_opacity(a); break;
-    case WRCU_KIND_TEXT_RUN: wr_setup_text_run(a); break;
-    case WRCU_KIND_CLIP_RECTANGLE: wr_setup_clip_rectangle(a); break;
-    case WRCU_KIND_CLIP_BOX_SHADOW: wr_setup_clip_box_shadow(a); break;
-    case WRCU_KIND_COMPOSITE:
-      if (features & WRCU_FEAT_YUV) wr_setup_composite_yuv(a);
-      else wr_setup_composite(a);
-      break;
-    case WRCU_KIND_CLEAR: wr_setup_clear(a); break;
-    case WRCU_KIND_BLUR: wr_setup_blur(a); break;
-    case WRCU_KIND_SCALE: wr_setup_scale(a); break;
-    case WRCU_KIND_FAST_LINEAR_GRADIENT: case WRCU_KIND_LINEAR_GRADIENT: case WRCU_KIND_RADIAL_GRADIENT:
-    case WRCU_KIND_CONIC_GRADIENT: wr_setup_cs_gradient(a); break;
-    case WRCU_KIND_LINE_DECORATION: wr_setup_line_decoration(a); break;
-    case WRCU_KIND_BORDER_SOLID: case WRCU_KIND_BORDER_SEGMENT: wr_setup_border(a); break;
-    case WRCU_KIND_QUAD_RADIAL_GRADIENT: case WRCU_KIND_QUAD_CONIC_GRADIENT: wr_setup_quad_gradient(a); break;
-    case WRCU_KIND_BRUSH_YUV_IMAGE: wr_setup_brush_yuv_image(a); break;
-    case WRCU_KIND_SPLIT_COMPOSITE: wr_setup_split_composite(a); break;
-    default: break;
+#ifndef WRCU_HOSTEMU
+__global__ void __launch_bounds__(128) wr_setup_multi(const SetupJob* jobs, const int* block_job, BatchInfo* reset, int n_reset,
+                                                      int* reset_ctr) {
+  __shared__ SetupJob sj;
+  if (blockIdx.x == 0) {  // re-arm the records the NEXT submission will use (the other half of the ring)
+    for (int i = threadIdx.x; i < n_reset; i += blockDim.x) wr_reset_batch_info(reset + i);
+    if (threadIdx.x < 2) reset_ctr[threadIdx.x] = 0;
   }
+  const int j = __ldg(block_job + blockIdx.x);
+  {
+    const uint4* src = (const uint4*)(jobs + j);
+    uint4* dst = (uint4*)&sj;
+    for (int i = threadIdx.x; i < (int)(sizeof(SetupJob) / 16); i += blockDim.x) dst[i] = __ldg(src + i);
+  }
+  __syncthreads();
+  wr_setup_batch(sj.kind, sj.features, sj.a, ((int)blockIdx.x - sj.first_block) * (int)blockDim.x + (int)threadIdx.x);
 }
 #endif
 
@@ -2345,7 +2197,7 @@ static int flush_pending(wrcu_ctx* c) {
     for (int i = 0; i < wrcu_ctx::QMAX; i++) wr_reset_batch_info(infos_next + i);
     ctr_next[0] = ctr_next[1] = 0;
     for (PendingOp& op : q)
-      if (op.type == 1) setup_host(op.kind, op.features, op.sa);
+      if (op.type == 1) wr_setup_batch(op.kind, op.features, op.sa, 0);
 #endif
   }
   c->launch_stream = c->stream;
@@ -2372,20 +2224,6 @@ static int flush_pending(wrcu_ctx* c) {
 
 extern "C" int wrcu_program_from_name(const char* key, int* kind, uint32_t* features) {
   if (!key || !kind || !features) return WRCU_ERR_INVALID;
-  static const struct { const char* name; int kind; } names[] = {
-      {"ps_quad_textured", WRCU_KIND_QUAD_TEXTURED}, {"ps_quad_mask", WRCU_KIND_QUAD_MASK},
-      {"brush_solid", WRCU_KIND_BRUSH_SOLID}, {"brush_image", WRCU_KIND_BRUSH_IMAGE},
-      {"brush_linear_gradient", WRCU_KIND_BRUSH_LINEAR_GRADIENT}, {"brush_blend", WRCU_KIND_BRUSH_BLEND},
-      {"brush_mix_blend", WRCU_KIND_BRUSH_MIX_BLEND}, {"brush_opacity", WRCU_KIND_BRUSH_OPACITY},
-      {"ps_text_run", WRCU_KIND_TEXT_RUN}, {"cs_clip_rectangle", WRCU_KIND_CLIP_RECTANGLE},
-      {"cs_clip_box_shadow", WRCU_KIND_CLIP_BOX_SHADOW}, {"composite", WRCU_KIND_COMPOSITE}, {"brush_yuv_image", WRCU_KIND_BRUSH_YUV_IMAGE},
-      {"ps_split_composite", WRCU_KIND_SPLIT_COMPOSITE},
-      {"ps_clear", WRCU_KIND_CLEAR}, {"cs_blur", WRCU_KIND_BLUR}, {"cs_scale", WRCU_KIND_SCALE},
-      {"cs_fast_linear_gradient", WRCU_KIND_FAST_LINEAR_GRADIENT}, {"cs_linear_gradient", WRCU_KIND_LINEAR_GRADIENT},
-      {"cs_radial_gradient", WRCU_KIND_RADIAL_GRADIENT}, {"cs_conic_gradient", WRCU_KIND_CONIC_GRADIENT},
-      {"cs_line_decoration", WRCU_KIND_LINE_DECORATION}, {"cs_border_solid", WRCU_KIND_BORDER_SOLID},
-      {"cs_border_segment", WRCU_KIND_BORDER_SEGMENT}, {"ps_quad_radial_gradient", WRCU_KIND_QUAD_RADIAL_GRADIENT},
-      {"ps_quad_conic_gradient", WRCU_KIND_QUAD_CONIC_GRADIENT}};
   static const struct { const char* name; uint32_t bit; } feats[] = {
       {"ALPHA_PASS", WRCU_FEAT_ALPHA_PASS}, {"FAST_PATH", WRCU_FEAT_FAST_PATH},
       {"ANTIALIASING", WRCU_FEAT_ANTIALIASING}, {"REPETITION", WRCU_FEAT_REPETITION},
@@ -2396,8 +2234,8 @@ extern "C" int wrcu_program_from_name(const char* key, int* kind, uint32_t* feat
   const char* sp = strchr(key, ' ');
   size_t nlen = sp ? (size_t)(sp - key) : strlen(key);
   *kind = 0;
-  for (auto& e : names)
-    if (strlen(e.name) == nlen && !strncmp(e.name, key, nlen)) *kind = e.kind;
+  for (int k = 1; k < N_KINDS; k++)
+    if (strlen(kinds[k].program) == nlen && !strncmp(kinds[k].program, key, nlen)) *kind = k;
   if (!*kind) return WRCU_ERR_UNSUPPORTED;
   *features = 0;
   const char* p = sp ? sp + 1 : nullptr;

@@ -2,7 +2,10 @@
 //
 // Layout of the implementation (all sm_90a CUDA, no CPU fallback):
 //   wrcu_api.cu      C ABI (include/wrcu.h): context, textures, frame tables,
-//                    target binding, clears, draw dispatch.
+//                    target binding, clears, draw dispatch.  What the draw
+//                    path knows about each program kind (WRCU_KIND_*) is one
+//                    row of its `kinds` table; wr_setup_batch picks the
+//                    kind's set-up.
 //   cmd.cuh          DrawCmd records produced by the per-kind "setup" kernels
 //                    (= the reference's vertex stage, one thread per instance).
 //   blend.cuh        The blend stage (bit-identical integer math to
