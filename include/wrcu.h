@@ -271,6 +271,14 @@ int wrcu_target_bind(wrcu_ctx* ctx, wrcu_tex color, wrcu_tex depth,
  * whole target; color NULL = leave colour; depth NULL = leave depth. */
 int wrcu_clear(wrcu_ctx* ctx, const int32_t rect[4], const float color[4],
                const float* depth);
+/* clear_target(color, None, Some(rect)) issued once per rect — the
+ * compositor clearing each part of the framebuffer that no opaque tile
+ * covers — in one queued op and one launch per 64 rects.  `rects` holds n
+ * x,y,w,h rects of the bound colour target (RGBA8 or R8); each is clamped
+ * like wrcu_clear's rect and empty ones are dropped (n = 0 queues nothing).
+ * The bytes written equal those of wrcu_clear called once per rect. */
+int wrcu_clear_rects(wrcu_ctx* ctx, const int32_t* rects, int n,
+                     const float color[4]);
 
 /* ---- draws ---------------------------------------------------------------- */
 /* draw_instanced_batch (renderer/mod.rs:2022-2065) =

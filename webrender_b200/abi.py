@@ -152,7 +152,7 @@ SYMBOLS = [
     "wrcu_last_error_string", "wrcu_get_string", "wrcu_abi_version",
     "wrcu_finish", "wrcu_texture_create", "wrcu_texture_set_filter",
     "wrcu_texture_upload", "wrcu_texture_destroy", "wrcu_read_pixels",
-    "wrcu_frame_begin", "wrcu_frame_end", "wrcu_target_bind", "wrcu_clear",
+    "wrcu_frame_begin", "wrcu_frame_end", "wrcu_target_bind", "wrcu_clear", "wrcu_clear_rects",
     "wrcu_draw_batch", "wrcu_draw_composite_tiles", "wrcu_program_from_name", "wrcu_get_stats",
     "wrcu_reset_stats", "wrcu_timer_begin", "wrcu_timer_end",
     "wrcu_texture_device_ptr", "wrcu_stream", "wrcu_host_alloc", "wrcu_host_free",

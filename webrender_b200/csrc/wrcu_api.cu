@@ -60,6 +60,7 @@ struct PendingOp {
   unsigned grid_x = 0, grid_y = 0;
   size_t bin_need = 0, inst_off = 0, views_off = (size_t)-1;
   std::vector<const uint8_t*> tex_reads;  // wrcu_draw_composite_tiles: the instances' textures (stream scheduling)
+  std::vector<int4> c_rects;              // wrcu_clear_rects: x0, y0, x1, y1 of each rect (at most WR_CLEAR_RECTS_MAX)
   SetupArgs sa;
   RasterArgs ra;
 };
@@ -140,6 +141,18 @@ __global__ void wr_clear_u8(uint8_t* base, int pitch, int x0, int y0, int x1, in
   for (int x = x0 + blockIdx.x * blockDim.x + threadIdx.x; x < x1; x += gridDim.x * blockDim.x) row[x] = v;
 }
 
+#endif
+
+// Rect-list clear (wrcu_clear_rects, clear_rects.cuh).  The kernels live in clear_rects.cu, their own
+// translation unit, so that adding them left the code generated for this file's kernels as it was.
+#include "clear_rects.cuh"
+#ifdef WRCU_HOSTEMU
+static void wr_clear_rects_u32(const ClearRects& p) {
+  for (int i = 0; i < p.n; i++) wr_clear_u32(p.base, p.pitch, p.r[i].x, p.r[i].y, p.r[i].z, p.r[i].w, p.v);
+}
+static void wr_clear_rects_u8(const ClearRects& p) {
+  for (int i = 0; i < p.n; i++) wr_clear_u8(p.base, p.pitch, p.r[i].x, p.r[i].y, p.r[i].z, p.r[i].w, (uint8_t)p.v);
+}
 #endif
 
 // ---- update path kernels (SURVEY.md §8f rank 3) -------------------------------------------
@@ -1364,11 +1377,8 @@ static int wait_pending_read(wrcu_ctx* c, WrTexture* t) {
   return rc;
 }
 
-extern "C" int wrcu_clear(wrcu_ctx* c, const int32_t rect[4], const float color[4], const float* depth) {
-  WrTexture* t = get_tex(c, c->color_tex);
-  if (!t) return wrcu_fail(c, WRCU_ERR_INVALID, "clear: no target bound");
-  cudaSetDevice(c->device);
-  { int rcw = wait_pending_read(c, t); if (rcw != WRCU_OK) return rcw; }
+// The rect x, y, w, h clamped to the target as x0, y0, x1, y1 (rect NULL = the whole target); false if empty.
+static bool clamp_clear_rect(const WrTexture* t, const int32_t* rect, int4* out) {
   int x0 = 0, y0 = 0, x1 = t->w, y1 = t->h;
   if (rect) {
     x0 = rect[0] > 0 ? rect[0] : 0;
@@ -1376,17 +1386,31 @@ extern "C" int wrcu_clear(wrcu_ctx* c, const int32_t rect[4], const float color[
     x1 = rect[0] + rect[2] < t->w ? rect[0] + rect[2] : t->w;
     y1 = rect[1] + rect[3] < t->h ? rect[1] + rect[3] : t->h;
   }
-  if (x1 <= x0 || y1 <= y0) return WRCU_OK;
+  *out = make_int4(x0, y0, x1, y1);
+  return x1 > x0 && y1 > y0;
+}
+
+// ClearTexSubImage: round_pixel, truncating U8 convert, BGRA swizzle (gl.cc:2426-2481)
+static uint32_t clear_color_value(int fmt, const float color[4]) {
+  uint32_t r = host_round_pixel(color[0]) & 0xFF, g = host_round_pixel(color[1]) & 0xFF;
+  uint32_t b = host_round_pixel(color[2]) & 0xFF, a = host_round_pixel(color[3]) & 0xFF;
+  return fmt == WRCU_FMT_RGBA8 ? (b | (g << 8) | (r << 16) | (a << 24)) : r;
+}
+
+extern "C" int wrcu_clear(wrcu_ctx* c, const int32_t rect[4], const float color[4], const float* depth) {
+  WrTexture* t = get_tex(c, c->color_tex);
+  if (!t) return wrcu_fail(c, WRCU_ERR_INVALID, "clear: no target bound");
+  cudaSetDevice(c->device);
+  { int rcw = wait_pending_read(c, t); if (rcw != WRCU_OK) return rcw; }
+  int4 cr;
+  if (!clamp_clear_rect(t, rect, &cr)) return WRCU_OK;
   // queued in order with the batches (flush_pending): a clear between two batches of a submission must stay there
   PendingOp op;
   op.type = 0;
-  op.cx0 = x0; op.cy0 = y0; op.cx1 = x1; op.cy1 = y1;
+  op.cx0 = cr.x; op.cy0 = cr.y; op.cx1 = cr.z; op.cy1 = cr.w;
   if (color) {
-    // ClearTexSubImage: round_pixel, truncating U8 convert, BGRA swizzle (gl.cc:2426-2481)
-    uint32_t r = host_round_pixel(color[0]) & 0xFF, g = host_round_pixel(color[1]) & 0xFF;
-    uint32_t b = host_round_pixel(color[2]) & 0xFF, a = host_round_pixel(color[3]) & 0xFF;
     op.c_ptr = t->dptr; op.c_pitch = (int)t->pitch; op.c_fmt = t->fmt;
-    op.c_val = t->fmt == WRCU_FMT_RGBA8 ? (b | (g << 8) | (r << 16) | (a << 24)) : r;
+    op.c_val = clear_color_value(t->fmt, color);
   }
   if (depth && c->depth_tex) {
     WrTexture* d = get_tex(c, c->depth_tex);
@@ -1399,7 +1423,65 @@ extern "C" int wrcu_clear(wrcu_ctx* c, const int32_t rect[4], const float color[
   return WRCU_OK;
 }
 
+// clear_target with a rect, issued once per rect: the rects (x, y, w, h) are clamped like wrcu_clear's,
+// empty ones dropped, and the rest queued as one clear op per WR_CLEAR_RECTS_MAX rects.
+extern "C" int wrcu_clear_rects(wrcu_ctx* c, const int32_t* rects, int n, const float color[4]) {
+  WrTexture* t = get_tex(c, c->color_tex);
+  if (!t) return wrcu_fail(c, WRCU_ERR_INVALID, "clear_rects: no target bound");
+  if (n < 0 || (n > 0 && !rects) || !color) return wrcu_fail(c, WRCU_ERR_INVALID, "clear_rects: bad rect list or colour");
+  if (t->fmt != WRCU_FMT_RGBA8 && t->fmt != WRCU_FMT_R8)
+    return wrcu_fail(c, WRCU_ERR_UNSUPPORTED, "clear_rects: target is neither RGBA8 nor R8");
+  cudaSetDevice(c->device);
+  { int rcw = wait_pending_read(c, t); if (rcw != WRCU_OK) return rcw; }
+  PendingOp op;
+  for (int i = 0; i <= n; i++) {
+    int4 cr;
+    if (i < n && !clamp_clear_rect(t, rects + 4 * (size_t)i, &cr)) continue;
+    if (i < n) {
+      if (op.c_rects.empty()) { op.cx0 = cr.x; op.cy0 = cr.y; op.cx1 = cr.z; op.cy1 = cr.w; }
+      op.cx0 = min(op.cx0, cr.x); op.cy0 = min(op.cy0, cr.y); op.cx1 = max(op.cx1, cr.z); op.cy1 = max(op.cy1, cr.w);
+      op.c_rects.push_back(cr);
+    }
+    if (op.c_rects.size() == (size_t)WR_CLEAR_RECTS_MAX || (i == n && !op.c_rects.empty())) {
+      op.type = 0;
+      op.c_ptr = t->dptr; op.c_pitch = (int)t->pitch; op.c_fmt = t->fmt;
+      op.c_val = clear_color_value(t->fmt, color);
+      pending(c).push_back(op);
+      op = PendingOp();
+      if (pending(c).size() >= (size_t)wrcu_ctx::QMAX || c->immediate) {
+        int rc = flush_pending(c);
+        if (rc != WRCU_OK) return rc;
+      }
+    }
+  }
+  return WRCU_OK;
+}
+
+static int launch_clear_rects(wrcu_ctx* c, const PendingOp& op) {
+  ClearRects p;
+  p.base = op.c_ptr; p.pitch = op.c_pitch; p.v = op.c_val;
+  p.n = (int)op.c_rects.size();
+  int rows = 0, wmax = 0;
+  for (int i = 0; i < p.n; i++) {
+    const int4 r = op.c_rects[(size_t)i];
+    p.r[i] = r;
+    p.row0[i] = rows;
+    rows += r.w - r.y;
+    wmax = max(wmax, r.z - r.x);
+  }
+  p.row0[p.n] = rows;
+  dim3 grid((unsigned)rows, (unsigned)min(8, (wmax + 1023) / 1024));
+  if (op.c_fmt == WRCU_FMT_RGBA8)
+    WR_LAUNCH(wr_clear_rects_u32, grid, 256, c->launch_stream, p);
+  else
+    WR_LAUNCH(wr_clear_rects_u8, grid, 256, c->launch_stream, p);
+  c->stats.kernel_launches++;
+  WRCU_CUDA(c, cudaGetLastError());
+  return WRCU_OK;
+}
+
 static int launch_clear(wrcu_ctx* c, const PendingOp& op) {
+  if (!op.c_rects.empty()) return launch_clear_rects(c, op);
   dim3 grid((unsigned)((op.cx1 - op.cx0 + 1023) / 1024), (unsigned)(op.cy1 - op.cy0));
   if (grid.x > 8) grid.x = 8;
   if (op.c_ptr) {

@@ -142,6 +142,14 @@ class DeviceBase:
         d = C.byref(C.c_float(depth)) if depth is not None else None
         self._check(self._f("clear")(self.ctx, r, col, C.cast(d, C.POINTER(C.c_float)) if d is not None else None))
 
+    def clear_rects(self, rects, color):
+        """wrcu_clear_rects: clear each (x, y, w, h) of `rects` to `color` (one launch per 64 rects)."""
+        rects = np.ascontiguousarray(np.asarray(rects, dtype=np.int32).reshape(-1, 4))
+        f = self._f("clear_rects")
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_float)]
+        self._check(f(self.ctx, rects.ctypes.data if len(rects) else None, len(rects),
+                      (C.c_float * 4)(*color)))
+
     def draw_batch(self, kind, features, blend, depth, colors, clip_mask, scissor, blend_color, inst):
         st = abi.DrawState()
         st.blend, st.depth = blend, depth

@@ -9,6 +9,9 @@ The converter classifies ops the way the frame builder would have placed them:
   * RGBA8 target, brush / text batches      → PictureCacheTarget (opaque batches = blend NONE + depth write,
                                               stored in batch order: the renderer draws them reversed)
   * RGBA8 target with only composite ops    → composite_simple (CompositeState tiles)
+
+A composite state can also be handed over directly (build_composite): tiles with their z order, valid and
+dirty rects, drawn with occlusion culling and, once set_partial_present enables it, partial present.
 """
 import ctypes as C
 import os
@@ -50,6 +53,24 @@ def _blend_mode(key):
     raise ValueError(f"blend key {key} has no BlendMode equivalent")
 
 
+TILE_OPAQUE, TILE_CLEAR, TILE_ALPHA = 0, 1, 2   # wr::CompositeTileKind
+
+
+class CompositeTile:
+    """One tile of a composite state (composite.rs CompositeTile).
+
+    kind: TILE_OPAQUE / TILE_CLEAR / TILE_ALPHA.  textures: one RGBA texture handle, or three YUV plane
+    handles (then `instance` is a composite_yuv_instance).  instance: the 120-byte CompositeInstance;
+    its rect is the device tile box, its clip rect the tile's device clip rect.  z_id: tiles are drawn in
+    ascending z_id, i.e. front to back.  valid_rect / dirty_rect: (x0, y0, x1, y1) in device pixels,
+    None = the instance's rect clipped to its clip rect."""
+
+    def __init__(self, kind, textures, instance, z_id, valid_rect=None, dirty_rect=None, fast_path=False):
+        self.kind, self.instance, self.z_id = kind, instance, z_id
+        self.textures = tuple(textures) if isinstance(textures, (tuple, list)) else (textures,)
+        self.valid_rect, self.dirty_rect, self.fast_path = valid_rect, dirty_rect, fast_path
+
+
 class NativeFrame:
     """A wr::Frame built by HostRenderer.build (owns the arrays its pointers refer to)."""
 
@@ -60,6 +81,25 @@ class NativeFrame:
         if self.ptr:
             self.hr.lib.wrh_frame_destroy(self.ptr)
             self.ptr = None
+
+
+def occlusion_build(lib, rects, opaque):
+    """wrh_occlusion_build through `lib` (libwrhost.so; needs no device).  See HostRenderer.occlusion_build."""
+    rects = np.ascontiguousarray(np.asarray(rects, dtype=np.float32).reshape(-1, 4))
+    op = np.ascontiguousarray(np.asarray(opaque, dtype=np.int32))
+    n = len(rects)
+    vis = np.zeros(max(1, 2 * n), np.int32)
+    n_opaque = C.c_int(0)
+    vp = C.c_void_p
+    lib.wrh_occlusion_build.argtypes = [vp, vp, C.c_int, vp, vp, vp, C.c_int, C.POINTER(C.c_int)]
+    total = 0
+    for cap in (0, None):   # count the items, then fetch them
+        cap = total if cap is None else cap
+        keys, items = np.zeros(max(1, cap), np.int32), np.zeros((max(1, cap), 4), np.float32)
+        total = lib.wrh_occlusion_build(rects.ctypes.data, op.ctypes.data, n, vis.ctypes.data, keys.ctypes.data,
+                                        items.ctypes.data, cap, C.byref(n_opaque))
+    out = [(int(keys[i]), tuple(float(v) for v in items[i])) for i in range(total)]
+    return out[:n_opaque.value], out[n_opaque.value:], vis[:n].astype(bool), vis[n:].astype(bool)
 
 
 class HostRenderer:
@@ -98,6 +138,12 @@ class HostRenderer:
         L.wrh_frame_add_composite_tile.argtypes = [vp, i32, u32, i32, C.POINTER(C.c_float)]
         L.wrh_frame_add_composite_yuv_tile.argtypes = [vp, i32, C.POINTER(u32), C.POINTER(C.c_float)]
         L.wrh_renderer_render.argtypes = [vp, vp, C.POINTER(C.c_uint64)]
+        f4 = C.POINTER(C.c_float)
+        L.wrh_composite_state_add_tile.argtypes = [vp, i32, C.POINTER(u32), i32, i32, f4, i32, f4, f4]
+        L.wrh_composite_state_set_dirty_rects_are_valid.argtypes = [vp, i32]
+        L.wrh_renderer_set_partial_present.argtypes = [vp, i32, i32]
+        L.wrh_renderer_render_with_age.argtypes = [vp, vp, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(i32), i32,
+                                                   C.POINTER(C.c_int)]
         L.wrh_renderer_last_error.restype = C.c_char_p
         L.wrh_renderer_last_error.argtypes = [vp]
         self.r = L.wrh_renderer_create(dev.ctx)
@@ -165,6 +211,39 @@ class HostRenderer:
             raise WrcuError(err, "RendererError: " + self.lib.wrh_renderer_last_error(self.r).decode())
         return calls.value
 
+    # -- composite state handed over directly ---------------------------------------------------------
+    def build_composite(self, fb, width, height, clear_color, tiles, dirty_rects_are_valid=True):
+        """A wr::Frame that only composites `tiles` (CompositeTile list) into the framebuffer texture `fb`
+        (clear_color None = no clear).  Render it with render_native or render_with_age."""
+        L = self.lib
+        f = L.wrh_frame_create(C.byref(abi.FrameTables()))
+        L.wrh_frame_set_framebuffer(f, fb, width, height, (C.c_float * 4)(*clear_color) if clear_color else None)
+        for t in tiles:
+            yuv = len(t.textures) == 3
+            planes = (C.c_uint32 * 3)(*(t.textures if yuv else (t.textures[0], 0, 0)))
+            inst = np.ascontiguousarray(t.instance).view(np.float32)
+            r4 = lambda r: (C.c_float * 4)(*r) if r is not None else None
+            L.wrh_composite_state_add_tile(f, t.kind, planes, 1 if yuv else 0, 1 if t.fast_path else 0,
+                                           (C.c_float * 30)(*inst), int(t.z_id), r4(t.valid_rect), r4(t.dirty_rect))
+        L.wrh_composite_state_set_dirty_rects_are_valid(f, 1 if dirty_rects_are_valid else 0)
+        return NativeFrame(self, f, {}, [])
+
+    def set_partial_present(self, max_partial_present_rects, draw_previous_partial_present_regions=False):
+        """The Draw compositor's partial-present settings (0 rects = redraw every frame whole)."""
+        self.lib.wrh_renderer_set_partial_present(self.r, max_partial_present_rects,
+                                                  1 if draw_previous_partial_present_regions else 0)
+
+    def render_with_age(self, nf, buffer_age):
+        """Renderer::render of a built frame into a back buffer `buffer_age` frames old (0 = new).
+        Returns (draw_calls, dirty_rects) with the rects as (x0, y0, x1, y1)."""
+        calls, n = C.c_uint64(0), C.c_int(0)
+        out = (C.c_int32 * 64)()
+        err = self.lib.wrh_renderer_render_with_age(self.r, nf.ptr, buffer_age, C.byref(calls), out, 16, C.byref(n))
+        self._pending_keep = []
+        if err != 0:
+            raise WrcuError(err, "RendererError: " + self.lib.wrh_renderer_last_error(self.r).decode())
+        return calls.value, [tuple(out[4 * i:4 * i + 4]) for i in range(min(n.value, 16))]
+
     def render(self, frame: Frame, handles=None):
         """Build the wr::Frame for `frame`, render it, return (handles, draw_calls)."""
         nf = self.build(frame, handles)
@@ -173,6 +252,12 @@ class HostRenderer:
         finally:
             nf.destroy()
         return nf.handles, calls
+
+    def occlusion_build(self, rects, opaque):
+        """The compositor's occlusion builder on `rects` (x0, y0, x1, y1 floats, front to back).  Returns
+        (opaque_items, alpha_items, tested, added): items as (key, rect) in the builder's order, `tested`
+        and `added` the per-rect results of test() just before add() and of add()."""
+        return occlusion_build(self.lib, rects, opaque)
 
     def _add_blur_scale(self, f, p, target_kind, t, b, handles, ptr, n):
         if b.kind == abi.KIND_SCALE:
@@ -235,15 +320,12 @@ class HostRenderer:
         if kinds and kinds <= {abi.KIND_COMPOSITE}:
             cc = clears[0].color if clears else None
             L.wrh_frame_set_framebuffer(f, tex, desc.width, desc.height, (C.c_float * 4)(*cc) if cc else None)
-            # the flat frame lists opaque tiles in draw order (front to back); CompositeState keeps z order
-            opaque = [b for b in batches if b.blend == abi.BLEND_NONE][::-1]
+            # listed in the flat frame's draw order: composite_simple draws them so, unsplit
+            opaque = [b for b in batches if b.blend == abi.BLEND_NONE]
             rest = [b for b in batches if b.blend != abi.BLEND_NONE]
             for b in opaque + rest:
                 kind = 0 if b.blend == abi.BLEND_NONE else (1 if b.blend == abi.BLEND_PREMULTIPLIED_DEST_OUT else 2)
-                a = b.instance_bytes()
-                if kind == 0:
-                    a = a[::-1]   # composite_simple walks opaque tiles front to back: keep the batch's draw order
-                for row in a:
+                for row in b.instance_bytes():
                     v = np.ascontiguousarray(row).view(np.float32)
                     if b.features & abi.FEAT_YUV:
                         planes = (C.c_uint32 * 3)(*[handles[nm] if nm else 0 for nm in b.color])

@@ -3,7 +3,10 @@
 // replace the GL calls there (INTEGRATION.md §2).
 #include "wr_renderer.h"
 
+#include <math.h>
 #include <string.h>
+
+#include <algorithm>
 
 namespace wr {
 
@@ -280,10 +283,12 @@ void Renderer::draw_texture_cache_target(const TextureCacheRenderTarget& t, Rend
   draw_blurs(t.horizontal_blurs, true, stats);
 }
 
-void Renderer::draw_tile_list(const std::vector<const CompositeTile*>& tiles, int blend, RendererStats& stats) {
+void Renderer::draw_tile_list(const std::vector<CompositeTile>& tiles, const std::vector<occlusion::Item>& items,
+                              int blend, RendererStats& stats) {
   // The reference breaks the instance list whenever the texture or the shader parameters change
   // (mod.rs:3289-3316) — a GL draw binds one sColor0.  wrcu_draw_composite_tiles carries the texture
   // per instance, so a run of tiles only breaks on the shader parameters (FAST_PATH; RGBA vs YUV).
+  // Pieces of one tile never overlap, so a run of them stays a copy-engine batch (BatchInfo::all_copy).
   state.blend = blend;
   std::vector<CompositeInstance> instances;
   std::vector<wrcu_tex> textures;
@@ -307,48 +312,157 @@ void Renderer::draw_tile_list(const std::vector<const CompositeTile*>& tiles, in
     instances.clear();
     textures.clear();
   };
-  for (const CompositeTile* t : tiles) {
+  for (const occlusion::Item& item : items) {
+    const CompositeTile* t = &tiles[item.key];
     bool brk = cur && (cur->fast_path != t->fast_path || cur->yuv != t->yuv);
     if (cur && t->yuv && !brk)
       brk = cur->texture != t->texture || cur->planes[0] != t->planes[0] || cur->planes[1] != t->planes[1];
     if (brk) flush();
     cur = t;
-    instances.push_back(t->instance);
+    CompositeInstance inst = t->instance;  // CompositeInstance::new(tile_rect, clip_rect = item.rectangle, ..)
+    inst.v[4] = item.rectangle.x0; inst.v[5] = item.rectangle.y0;
+    inst.v[6] = item.rectangle.x1; inst.v[7] = item.rectangle.y1;
+    instances.push_back(inst);
     textures.push_back(t->texture);
   }
   flush();
 }
 
-void Renderer::composite_simple(const Frame& frame, RendererStats& stats) {
+static bool whole_pixels(const DeviceBox2D& r) {
+  return floorf(r.x0) == r.x0 && floorf(r.y0) == r.y0 && floorf(r.x1) == r.x1 && floorf(r.y1) == r.y1;
+}
+
+void Renderer::composite_simple(const Frame& frame, const std::optional<PartialPresentMode>& partial_present_mode,
+                                RendererStats& stats) {
   bind_draw_target(frame.framebuffer, 0, frame.fb_width, frame.fb_height);
   state.depth = WRCU_DEPTH_OFF;
   state.scissor_enabled = 0;
   const CompositeState& cs = frame.composite_state;
-  if (cs.has_clear_color && wrcu_clear(device, nullptr, cs.clear_color, nullptr) != WRCU_OK) failed++;
-  // opaque tiles front to back with blending off, then clear tiles (dest-out), then alpha
-  // tiles back to front (mod.rs:3417-3470); occlusion splitting happened upstream.
-  std::vector<const CompositeTile*> opaque, clear, alpha;
-  for (const CompositeTile& t : cs.tiles) {
-    if (t.kind == CompositeTileKind::Opaque) opaque.insert(opaque.begin(), &t);
-    else if (t.kind == CompositeTileKind::Clear) clear.push_back(&t);
-    else alpha.push_back(&t);
+  // front to back (CompositeState::end_frame, composite.rs:1021), or as listed
+  std::vector<size_t> order(cs.tiles.size());
+  for (size_t i = 0; i < order.size(); i++) order[i] = i;
+  if (!cs.listed)
+    std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return cs.tiles[a].z_id < cs.tiles[b].z_id; });
+
+  occlusion::FrontToBackBuilder occlusion;
+  std::vector<occlusion::Item> opaque, clear_tiles, alpha;  // in draw order
+  for (size_t idx : order) {
+    const CompositeTile& tile = cs.tiles[idx];
+    const DeviceBox2D device_tile_box = tile.device_box();
+    const DeviceBox2D partial_clip_rect = partial_present_mode ? partial_present_mode->dirty_rect : device_tile_box;
+    const DeviceBox2D rect = device_tile_box.intersection_unchecked(tile.clip_rect())
+                                 .intersection_unchecked(partial_clip_rect)
+                                 .intersection_unchecked(tile.valid_rect);
+    if (rect.is_empty()) continue;
+    // Clear tiles overwrite what is under them, but with their own blend state: drawn after the opaque
+    // tiles and before the alpha ones, outside the occlusion lists.
+    if (tile.kind == CompositeTileKind::Clear) clear_tiles.push_back(occlusion::Item{rect, idx});
+    else if (cs.listed) (tile.kind == CompositeTileKind::Opaque ? opaque : alpha).push_back(occlusion::Item{rect, idx});
+    else occlusion.add(rect, tile.kind == CompositeTileKind::Opaque, idx);
   }
-  if (!opaque.empty()) draw_tile_list(opaque, WRCU_BLEND_NONE, stats);
-  if (!clear.empty()) draw_tile_list(clear, WRCU_BLEND_PREMULTIPLIED_DEST_OUT, stats);
-  if (!alpha.empty()) draw_tile_list(alpha, WRCU_BLEND_PREMULTIPLIED_ALPHA, stats);
+  if (!cs.listed) {
+    opaque = occlusion.opaque_items();
+    alpha.assign(occlusion.alpha_items().rbegin(), occlusion.alpha_items().rend());  // back to front
+  }
+
+  // The reference clears the framebuffer, or the dirty rect unless it is fully hidden (mod.rs:3420-3445).
+  // Of that region only what no opaque item covers is cleared: an opaque item with whole-pixel edges
+  // writes every pixel of its rect with blending off, so clearing those pixels first changes nothing.
+  // A fractional item may leave its edge pixels untouched, so its rect stays in the clear.
+  if (cs.has_clear_color) {
+    std::vector<DeviceBox2D> region;
+    const DeviceBox2D fb{0.0f, 0.0f, (float)frame.fb_width, (float)frame.fb_height};
+    if (!partial_present_mode) {
+      region.push_back(fb);
+    } else {
+      const DeviceBox2D& d = partial_present_mode->dirty_rect;
+      if (!d.is_empty() && (cs.listed || occlusion.test(d))) {  // DeviceRect::to_i32 truncates
+        const DeviceBox2D di{(float)(int32_t)d.x0, (float)(int32_t)d.y0, (float)(int32_t)d.x1, (float)(int32_t)d.y1};
+        const DeviceBox2D r = di.intersection_unchecked(fb);
+        if (!r.is_empty()) region.push_back(r);
+      }
+    }
+    for (const occlusion::Item& it : opaque) {
+      if (region.empty()) break;
+      if (whole_pixels(it.rectangle)) occlusion::apply_occluder(it.rectangle, region);
+    }
+    if (!region.empty()) {
+      std::vector<int32_t> rects;
+      for (const DeviceBox2D& r : region)
+        rects.insert(rects.end(), {(int32_t)r.x0, (int32_t)r.y0, (int32_t)(r.x1 - r.x0), (int32_t)(r.y1 - r.y0)});
+      if (wrcu_clear_rects(device, rects.data(), (int)region.size(), cs.clear_color) != WRCU_OK) failed++;
+    }
+  }
+
+  // opaque items front to back with blending off, then clear tiles (dest-out), then alpha items back to
+  // front (mod.rs:3447-3483)
+  if (!opaque.empty()) draw_tile_list(cs.tiles, opaque, WRCU_BLEND_NONE, stats);
+  if (!clear_tiles.empty()) draw_tile_list(cs.tiles, clear_tiles, WRCU_BLEND_PREMULTIPLIED_DEST_OUT, stats);
+  if (!alpha.empty()) draw_tile_list(cs.tiles, alpha, WRCU_BLEND_PREMULTIPLIED_ALPHA, stats);
   state.blend = WRCU_BLEND_NONE;
 }
 
-void Renderer::draw_frame(const Frame& frame, RendererStats& stats) {
+void BufferDamageTracker::push_dirty_rect(const DeviceBox2D& rect) {
+  damage_rects[current_offset] = rect;
+  current_offset = current_offset == 0 ? 3 : current_offset - 1;
+}
+
+std::optional<DeviceBox2D> BufferDamageTracker::get_damage_rect(size_t buffer_age) const {
+  if (buffer_age == 0) return std::nullopt;           // a new buffer: nothing in it is valid
+  if (buffer_age == 1) return DeviceBox2D{};          // last frame's back buffer: all valid
+  if (buffer_age > 5) return std::nullopt;            // older than the frames tracked
+  DeviceBox2D r;                                      // the frames drawn since it was the back buffer
+  for (size_t k = 0; k < buffer_age - 1; k++) r = r.union_with(damage_rects[(current_offset + 1 + k) % 4]);
+  return r;
+}
+
+static DeviceBox2D round_box(const DeviceBox2D& r) {  // euclid Box2D::round
+  return DeviceBox2D{floorf(r.x0 + 0.5f), floorf(r.y0 + 0.5f), floorf(r.x1 + 0.5f), floorf(r.y1 + 0.5f)};
+}
+
+// calculate_dirty_rects (mod.rs:4311-4416) for the Draw compositor with a partial-present interface
+std::optional<PartialPresentMode> Renderer::calculate_dirty_rects(size_t buffer_age, const CompositeState& cs,
+                                                                  int fb_width, int fb_height, RenderResults& results) {
+  std::optional<PartialPresentMode> mode;
+  if (partial_present.max_partial_present_rects <= 0) return mode;
+  const bool draw_previous = partial_present.draw_previous_partial_present_regions;
+  const DeviceBox2D fb_rect{0.0f, 0.0f, (float)fb_width, (float)fb_height};
+  const DeviceBox2D prev_frames_damage_rect = buffer_damage_tracker.get_damage_rect(buffer_age).value_or(fb_rect);
+  if (cs.dirty_rects_are_valid && !force_redraw) {
+    DeviceBox2D combined;
+    for (const CompositeTile& tile : cs.tiles) {
+      if (tile.kind == CompositeTileKind::Clear) continue;
+      const DeviceBox2D d = tile.dirty_rect.intersection_unchecked(fb_rect);
+      if (!d.is_empty()) combined = combined.union_with(d);
+    }
+    combined = round_box(combined);
+    if (!combined.is_empty())
+      results.dirty_rects.push_back(DeviceIntRect{(int32_t)combined.x0, (int32_t)combined.y0, (int32_t)combined.x1,
+                                                  (int32_t)combined.y1});
+    if (draw_previous) buffer_damage_tracker.push_dirty_rect(combined);
+    mode = PartialPresentMode{draw_previous ? combined.union_with(prev_frames_damage_rect) : combined};
+  } else {
+    results.dirty_rects.push_back(DeviceIntRect{0, 0, fb_width, fb_height});
+    if (draw_previous) buffer_damage_tracker.push_dirty_rect(fb_rect);
+  }
+  force_redraw = false;
+  return mode;
+}
+
+void Renderer::draw_frame(const Frame& frame, size_t buffer_age, RenderResults& results) {
   // bind_frame_data + gpu buffers + gpu cache (mod.rs:4418, 4551-4558) in one call
   if (wrcu_frame_begin(device, &frame.tables) != WRCU_OK) { failed++; return; }
+  std::optional<PartialPresentMode> present_mode;
+  if (frame.present)
+    present_mode = calculate_dirty_rects(buffer_age, frame.composite_state, frame.fb_width, frame.fb_height, results);
   for (const RenderPass& pass : frame.passes) {
-    for (const TextureCacheRenderTarget& t : pass.texture_cache) draw_texture_cache_target(t, stats);
-    for (const PictureCacheTarget& t : pass.picture_cache) draw_picture_cache_target(t, stats);
-    for (const AlphaRenderTarget& t : pass.alpha) draw_alpha_target(t, stats);
-    for (const ColorRenderTarget& t : pass.color) draw_color_target(t, stats);
+    for (const TextureCacheRenderTarget& t : pass.texture_cache) draw_texture_cache_target(t, results.stats);
+    for (const PictureCacheTarget& t : pass.picture_cache) draw_picture_cache_target(t, results.stats);
+    for (const AlphaRenderTarget& t : pass.alpha) draw_alpha_target(t, results.stats);
+    for (const ColorRenderTarget& t : pass.color) draw_color_target(t, results.stats);
   }
-  if (frame.present) composite_simple(frame, stats);
+  if (frame.present) composite_simple(frame, present_mode, results.stats);
+  else force_redraw = true;  // a frame drawn but not presented leaves the partial-present state unknown (mod.rs:4914)
   if (wrcu_frame_end(device) != WRCU_OK) failed++;
 }
 
@@ -410,13 +524,20 @@ RendererError Renderer::check_gl_errors() {
   return RendererError::None;
 }
 
-RendererError Renderer::render(const Frame& frame, RendererStats* stats) {
-  RendererStats local;
+RendererError Renderer::render(const Frame& frame, size_t buffer_age, RenderResults* results) {
+  RenderResults local;
   // render_impl (mod.rs:1441-1560): resource updates first, then the frame
   update_texture_cache();
   update_gpu_cache();
-  draw_frame(frame, stats ? *stats : local);
+  draw_frame(frame, buffer_age, results ? *results : local);
   return check_gl_errors();
+}
+
+RendererError Renderer::render(const Frame& frame, RendererStats* stats) {
+  RenderResults results;
+  RendererError e = render(frame, 0, &results);
+  if (stats) *stats = results.stats;
+  return e;
 }
 
 }  // namespace wr
@@ -552,13 +673,21 @@ void wrh_frame_set_framebuffer(Frame* f, wrcu_tex fb, int w, int h, const float*
   f->composite_state.has_clear_color = clear_color != nullptr;
   if (clear_color) memcpy(f->composite_state.clear_color, clear_color, 16);
 }
+// Tiles added by these two are drawn as listed, unsplit: opaque tiles in the order added, then clear
+// tiles, then alpha tiles, each in the order added (a flat frame's painter's order).  Their valid and
+// dirty rects are the instance's rect clipped to its clip rect.
+static void add_listed_tile(Frame* f, CompositeTile& t) {
+  t.valid_rect = t.dirty_rect = t.device_box().intersection_unchecked(t.clip_rect());
+  f->composite_state.listed = true;
+  f->composite_state.tiles.push_back(t);
+}
 void wrh_frame_add_composite_tile(Frame* f, int kind, wrcu_tex texture, int fast_path, const float* instance30) {
   CompositeTile t;
   t.kind = (CompositeTileKind)kind;
   t.texture = texture;
   t.fast_path = fast_path != 0;
   memcpy(t.instance.v, instance30, sizeof t.instance.v);
-  f->composite_state.tiles.push_back(t);
+  add_listed_tile(f, t);
 }
 void wrh_frame_add_composite_yuv_tile(Frame* f, int kind, const wrcu_tex* planes3, const float* instance30) {
   CompositeTile t;
@@ -568,7 +697,74 @@ void wrh_frame_add_composite_yuv_tile(Frame* f, int kind, const wrcu_tex* planes
   t.planes[0] = planes3[1];
   t.planes[1] = planes3[2];
   memcpy(t.instance.v, instance30, sizeof t.instance.v);
+  add_listed_tile(f, t);
+}
+// A tile of the composite state with its place and rects given (CompositeTile, composite.rs):
+//   kind: 0 opaque, 1 clear, 2 alpha; yuv = 0: planes3[0] is the RGBA texture (fast_path as above),
+//   yuv = 1: planes3 are the three planes; instance30: the CompositeInstance, whose rect is the device
+//   tile box and whose clip rect the tile's device clip rect; z_id: tiles are drawn in ascending z_id,
+//   front to back (ties keep the order of addition); valid_rect4 / dirty_rect4: x0, y0, x1, y1 in
+//   device pixels, NULL = the instance's rect clipped to its clip rect.
+void wrh_composite_state_add_tile(Frame* f, int kind, const wrcu_tex* planes3, int yuv, int fast_path,
+                                  const float* instance30, int32_t z_id, const float* valid_rect4,
+                                  const float* dirty_rect4) {
+  CompositeTile t;
+  t.kind = (CompositeTileKind)kind;
+  t.texture = planes3[0];
+  t.yuv = yuv != 0;
+  if (t.yuv) { t.planes[0] = planes3[1]; t.planes[1] = planes3[2]; }
+  t.fast_path = !t.yuv && fast_path != 0;
+  memcpy(t.instance.v, instance30, sizeof t.instance.v);
+  t.z_id = z_id;
+  const DeviceBox2D drawn = t.device_box().intersection_unchecked(t.clip_rect());
+  t.valid_rect = valid_rect4 ? DeviceBox2D{valid_rect4[0], valid_rect4[1], valid_rect4[2], valid_rect4[3]} : drawn;
+  t.dirty_rect = dirty_rect4 ? DeviceBox2D{dirty_rect4[0], dirty_rect4[1], dirty_rect4[2], dirty_rect4[3]} : drawn;
   f->composite_state.tiles.push_back(t);
+}
+void wrh_composite_state_set_dirty_rects_are_valid(Frame* f, int valid) {
+  f->composite_state.dirty_rects_are_valid = valid != 0;
+}
+// CompositorConfig::Draw's max_partial_present_rects / draw_previous_partial_present_regions
+void wrh_renderer_set_partial_present(Renderer* r, int max_partial_present_rects,
+                                      int draw_previous_partial_present_regions) {
+  r->partial_present.max_partial_present_rects = max_partial_present_rects;
+  r->partial_present.draw_previous_partial_present_regions = draw_previous_partial_present_regions != 0;
+}
+// Renderer::render with the back buffer's age.  Up to `cap` dirty rects (x0, y0, x1, y1) go to
+// dirty_rects4; *n_dirty receives how many the frame has.  Returns RendererError as int.
+int wrh_renderer_render_with_age(Renderer* r, const Frame* f, uint64_t buffer_age, uint64_t* draw_calls,
+                                 int32_t* dirty_rects4, int cap, int* n_dirty) {
+  RenderResults results;
+  RendererError e = r->render(*f, (size_t)buffer_age, &results);
+  if (draw_calls) *draw_calls = results.stats.total_draw_calls;
+  if (n_dirty) *n_dirty = (int)results.dirty_rects.size();
+  for (int i = 0; i < cap && i < (int)results.dirty_rects.size(); i++) {
+    const DeviceIntRect& d = results.dirty_rects[(size_t)i];
+    dirty_rects4[4 * i] = d.x0; dirty_rects4[4 * i + 1] = d.y0; dirty_rects4[4 * i + 2] = d.x1; dirty_rects4[4 * i + 3] = d.y1;
+  }
+  return (int)e;
+}
+// Test hook: FrontToBackBuilder over n rects (x0, y0, x1, y1) added front to back, rect i opaque when
+// opaque[i].  visible[i] receives test(rect i) just before add(rect i), visible[n + i] what add returned.
+// The opaque items, then the alpha items, go to keys / items4 (at most cap); returns how many items there
+// are in all, with the opaque count in *n_opaque.
+int wrh_occlusion_build(const float* rects4, const int32_t* opaque, int n, int32_t* visible, int32_t* keys,
+                        float* items4, int cap, int* n_opaque) {
+  occlusion::FrontToBackBuilder b;
+  for (int i = 0; i < n; i++) {
+    const DeviceBox2D r{rects4[4 * i], rects4[4 * i + 1], rects4[4 * i + 2], rects4[4 * i + 3]};
+    visible[i] = b.test(r) ? 1 : 0;
+    visible[n + i] = b.add(r, opaque[i] != 0, (size_t)i) ? 1 : 0;
+  }
+  std::vector<occlusion::Item> all(b.opaque_items());
+  all.insert(all.end(), b.alpha_items().begin(), b.alpha_items().end());
+  *n_opaque = (int)b.opaque_items().size();
+  for (int i = 0; i < cap && i < (int)all.size(); i++) {
+    keys[i] = (int32_t)all[(size_t)i].key;
+    const DeviceBox2D& r = all[(size_t)i].rectangle;
+    items4[4 * i] = r.x0; items4[4 * i + 1] = r.y0; items4[4 * i + 2] = r.x1; items4[4 * i + 3] = r.y1;
+  }
+  return (int)all.size();
 }
 // returns RendererError as int; *draw_calls receives RendererStats.total_draw_calls
 // update path: queue a GpuCacheUpdateList / texture updates for the next render

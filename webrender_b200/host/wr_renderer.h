@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "../../include/wrcu.h"
+#include "occlusion.h"
 
 namespace wr {
 
@@ -144,17 +145,47 @@ enum class CompositeTileKind { Opaque, Clear, Alpha };
 struct CompositeTile {
   CompositeTileKind kind = CompositeTileKind::Opaque;
   wrcu_tex texture = 0;   // picture-cache texture, external surface, or the 1x1 dummy
-  CompositeInstance instance;
+  CompositeInstance instance;  // v[0..3] the device tile box, v[4..7] its device clip rect
   bool fast_path = false; // NO_UV_CLAMP | NO_COLOR_MODULATION (composite.rs get_rgb_features)
   // ResolvedExternalSurfaceColorData::Yuv (composite.rs): CompositeSurfaceFormat::Yuv, planes in
   // sColor0..2 (BatchTextures::composite_yuv); `texture` is plane 0
   bool yuv = false;
   wrcu_tex planes[2] = {0, 0};  // planes 1 and 2
+  // CompositeTile::z_id: tiles are culled and drawn in ascending z_id, i.e. front to back (composite.rs:1021
+  // sorts them so); equal ids keep the order they were added in
+  int32_t z_id = 0;
+  DeviceBox2D valid_rect, dirty_rect;  // local_valid_rect / local_dirty_rect mapped to device space
+  DeviceBox2D device_box() const { return DeviceBox2D{instance.v[0], instance.v[1], instance.v[2], instance.v[3]}; }
+  DeviceBox2D clip_rect() const { return DeviceBox2D{instance.v[4], instance.v[5], instance.v[6], instance.v[7]}; }
 };
 struct CompositeState {
-  std::vector<CompositeTile> tiles;  // in z order (back to front)
+  std::vector<CompositeTile> tiles;
   bool has_clear_color = true;
   float clear_color[4] = {0, 0, 0, 0};
+  bool dirty_rects_are_valid = true;  // false: the tiles' dirty rects say nothing; present everything
+  // Tiles given in draw order (wrh_frame_add_composite_tile): drawn unsplit as listed, no occlusion
+  // culling.  Splitting a tile that is scaled, filtered or placed off the pixel grid changes where its
+  // rows start sampling, and so its bytes, against a frame that draws the tiles whole.
+  bool listed = false;
+};
+
+// PartialPresentMode::Single (mod.rs:440-452): only `dirty_rect` of the framebuffer is redrawn
+struct PartialPresentMode { DeviceBox2D dirty_rect; };
+
+// The Draw compositor's partial-present settings (CompositorConfig::Draw, composite.rs)
+struct PartialPresentConfig {
+  int max_partial_present_rects = 0;                  // 0 = no partial present: every frame is redrawn whole
+  bool draw_previous_partial_present_regions = false; // the host keeps no copy: redraw what older frames changed
+};
+
+// BufferDamageTracker (mod.rs:720-762): the dirty rects of the last four frames, so that a back buffer
+// `buffer_age` frames old can be brought up to date
+struct BufferDamageTracker {
+  DeviceBox2D damage_rects[4];
+  size_t current_offset = 0;
+  void push_dirty_rect(const DeviceBox2D& rect);
+  // empty = the buffer is up to date; nullopt = every pixel of it is stale
+  std::optional<DeviceBox2D> get_damage_rect(size_t buffer_age) const;
 };
 
 struct Frame {  // frame_builder.rs:1129 (members the path reads)
@@ -194,14 +225,21 @@ enum class RendererError { None, Shader, Thread, MaxTextureSize, SoftwareRasteri
 struct RendererStats {  // mod.rs RendererStats
   size_t total_draw_calls = 0, alpha_target_count = 0, color_target_count = 0;
 };
+struct RenderResults {  // mod.rs RenderResults (members the path fills)
+  RendererStats stats;
+  std::vector<DeviceIntRect> dirty_rects;  // what changed on screen this frame; none = nothing to present
+};
 
 class Renderer {
  public:
   explicit Renderer(wrcu_ctx* device) : device(device) {}
   // Renderer::render → render_impl → draw_frame (mod.rs:1241, 1441, 4525)
   RendererError render(const Frame& frame, RendererStats* stats);
+  // The same with the back buffer's age (frames since it was last the back buffer; 0 = new) for
+  // partial present: results->dirty_rects receives the frame's dirty rects.
+  RendererError render(const Frame& frame, size_t buffer_age, RenderResults* results);
 
-  void draw_frame(const Frame& frame, RendererStats& stats);
+  void draw_frame(const Frame& frame, size_t buffer_age, RenderResults& results);
   void draw_picture_cache_target(const PictureCacheTarget& target, RendererStats& stats);         // mod.rs:2669
   void draw_color_target(const ColorRenderTarget& target, RendererStats& stats);                  // mod.rs:3486
   void draw_alpha_target(const AlphaRenderTarget& target, RendererStats& stats);                  // mod.rs:3754
@@ -210,8 +248,16 @@ class Renderer {
   void draw_clip_batch_list(const ClipBatchList& list, int blend, RendererStats& stats);          // mod.rs:3695
   void draw_blurs(const BlurMap& blurs, bool color_target, RendererStats& stats);                 // mod.rs:3675
   void handle_scaling(const ScalingMap& scalings, RendererStats& stats);                          // mod.rs:2472
-  void composite_simple(const Frame& frame, RendererStats& stats);                                // mod.rs:3340
-  void draw_tile_list(const std::vector<const CompositeTile*>& tiles, int blend, RendererStats& stats);  // mod.rs:3126
+  void composite_simple(const Frame& frame, const std::optional<PartialPresentMode>& partial_present_mode,
+                        RendererStats& stats);                                                    // mod.rs:3340
+  // mod.rs:3126; each item is drawn with its tile's instance, clipped to the item's rectangle
+  void draw_tile_list(const std::vector<CompositeTile>& tiles, const std::vector<occlusion::Item>& items, int blend,
+                      RendererStats& stats);
+  std::optional<PartialPresentMode> calculate_dirty_rects(size_t buffer_age, const CompositeState& cs, int fb_width,
+                                                          int fb_height, RenderResults& results);  // mod.rs:4311
+  PartialPresentConfig partial_present;
+  BufferDamageTracker buffer_damage_tracker;
+  bool force_redraw = true;  // the next frame is presented whole (init.rs:782)
   // draw_instanced_batch<T> (mod.rs:2022-2065)
   void draw_instanced_batch(int kind, uint32_t features, const void* instances, size_t stride, size_t n,
                             const BatchTextures& textures, RendererStats& stats);
